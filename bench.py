@@ -1,6 +1,7 @@
-"""bench.py -- collocation-points/sec for one residual+gradient evaluation (BASELINE.json metric) on N B200s.
+"""bench.py -- collocation-points/sec for one residual+gradient evaluation (BASELINE.json metric) on N H100s.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2] [--points P] [--impl ours|reference]
+                  [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic collocation points: K0 pack -> K1 (forward jets +
 residual + seeds) -> loss finalize -> K2 (reverse pass) -> K2b (reduce); with N > 1 GPUs every rank owns its own
@@ -17,13 +18,18 @@ float64 = the reference's default dtype) on this box's host cores for the same w
 
 Besides the contract's keys the line carries, at N = 1: `cpu_baseline` (the same oracle closure on a bounded sample),
 `gpu_autograd_baseline` (the reference algorithm through stock PyTorch CUDA autograd on this GPU -- what a user of the
-reference gets on a B200 today) and `fit` (the product's Solver.fit end to end: host sampling, H2D, K0..K2b, Adam,
+reference gets on it today) and `fit` (the product's Solver.fit end to end: host sampling, H2D, K0..K2b, Adam,
 one loss read per epoch).  All three run AFTER the timed region.
+
+`--dump-outputs DIR` writes what the timed path computed in its last timed step -- the flat parameter gradient
+(`grad.npy`, float32) and the loss (`loss.npy`, float64) -- so that two builds can be compared output for output: with
+the same arguments the inputs (seeded network initialisation and points) are identical from run to run.
 """
 import argparse
 import json
 import os
 import sys
+import tempfile
 import threading
 import time
 
@@ -31,6 +37,9 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
+# the specialised forward kernel is compiled at run time and cached (default ~/.cache/pinnjet_jit); the bench may run
+# where HOME is absent or not writable, so unless the caller chose a cache it goes to the temporary directory
+os.environ.setdefault("PINNJET_JIT_CACHE", os.path.join(tempfile.gettempdir(), f"pinnjet_jit_{os.getuid()}"))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
@@ -52,6 +61,8 @@ def parse():
     ap.add_argument("--no-gpu-comparator", action="store_true", help="skip the torch-CUDA-autograd comparator leg")
     ap.add_argument("--no-graph", action="store_true", help="launch the step eagerly instead of replaying a CUDA graph")
     ap.add_argument("--no-strong", action="store_true", help="skip the C3 / C5 strong-scaling legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the gradient and loss of the last timed step to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -81,7 +92,7 @@ def _oracle_step_fn(key, n_points, dtype, device="cpu"):
 
 def gpu_autograd_comparator(key, n_points, dev, seconds=2.0):
     """Secondary comparator (SURVEY.md §8d): the SAME reference algorithm on the SAME GPU through stock PyTorch CUDA
-    autograd (what a user of the reference gets on a B200 today).  Baseline only, measured after the timed region."""
+    autograd (what a user of the reference gets on it today).  Baseline only, measured after the timed region."""
     out = {}
     for name, dtype in (("f32", torch.float32), ("f64", torch.float64)):
         step = _oracle_step_fn(key, n_points, dtype, device=dev)
@@ -346,12 +357,8 @@ def executed_flops(wl, tp):
 
 
 def load_peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            d = json.load(f)
-        return d.get("bf16_tflops", 1590.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+    """Dense BF16 tensor rate and HBM3 bandwidth of the H100 SXM data sheet (700 W card): a ceiling, not a measurement."""
+    return 989.0, 3350.0, "H100 SXM data sheet"
 
 
 def main():
@@ -384,7 +391,7 @@ def main():
 
     def flush_l2():
         """Write a 256 MiB buffer (evicts everything), then stream another 256 MiB through L2 by READING it so that the
-        cache is left full of CLEAN lines: a memset alone leaves 126 MB of dirty lines whose write-back would be charged
+        cache is left full of CLEAN lines: a memset alone leaves the L2 (50 MB on the H100) full of dirty lines whose write-back would be charged
         to the first kernel of the timed step."""
         flush.zero_()
         if os.environ.get("PINNJET_BENCH_DIRTY_FLUSH") != "1":
@@ -473,6 +480,10 @@ def main():
     ms_per_step = total_ms / args.steps
     value = n_global / (ms_per_step * 1e-3)
     loss = float(fp.sumsq.item()) / (n_global * fp.n_eq)
+    if args.dump_outputs and rank == 0:   # before anything below reuses the buffers
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "grad.npy"), fp.grad.detach().float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "loss.npy"), np.array([loss], dtype=np.float64))
 
     # ---- per-kernel timing for the roofline (events around each launch, same stream) ---------------------------------
     info = fp.plan_info(n)
@@ -590,29 +601,22 @@ def main():
     clocks = clk.summary()
     flops_k1 = wl.flops_fwdjet * n
     ach_k1 = flops_k1 / (k1_ms * 1e-3) / 1e12
-    sm_mhz = clocks.get("sm_mhz") or 1965.0
+    sm_mhz = clocks.get("sm_mhz") or clocks.get("sm_max_mhz") or 1980.0
     n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
     fp32_peak = n_sms * 128 * 2 * sm_mhz * 1e6 / 1e12       # FFMA lanes x 2 flop x clock under load
     tc_fwd, tc_bwd = bool(info.get("tc")), bool(info.get("tc_bwd"))
     k1_name = "k1tc3_forward_kernel" if tc_fwd else "k1_forward_kernel"
     k2_name = "k2tc2_backward_kernel" if tc_bwd else "k2_backward_kernel"
-    # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant kernel, from the committed `ncu --set full`
-    # capture of the same kernel variant (profiles/r02/traffic.json names the report it was read from); null if none.
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r02", "traffic.json")
-    if os.path.exists(tpath):
-        with open(tpath) as f:
-            traffic = json.load(f).get(args.workload, {}).get("pj_k1_jit" if (jit_on and tc_fwd) else k1_name, {}).get("dram_bytes")
     roofline = {
         "kernel": k1_name + (" specialised (pj_k1_jit: residual programs compiled in)" if jit_on else "") +
                   " (forward + jets + residual program)",
         "bound": "tensor", "achieved": ach_k1,
-        "peak": bf16_peak, "unit": "TFLOP/s", "frac": ach_k1 / bf16_peak, "traffic": traffic,
+        "peak": bf16_peak, "unit": "TFLOP/s", "frac": ach_k1 / bf16_peak,
         "peak_source": f"dense bf16 tensor, {peak_src}",
-        "pipe": ("tcgen05.mma kind::f16, bf16x3 split operands (6 bf16 products per fp32 product, fp32 TMEM accumulators): "
+        "pipe": ("wgmma m64n16k16 bf16, bf16x3 split operands (6 bf16 products per fp32 product, fp32 register accumulators): "
                  "hidden-layer and output contractions on the tensor pipe; layer 0, activation jets and the residual program "
                  "on the CUDA cores" if tc_fwd else
-                 "fp32 FFMA2 on CUDA cores (network not eligible for the tensor-core kernels: hidden width != 64, "
+                 "fp32 FFMA on CUDA cores (network not eligible for the tensor-core kernels: hidden width != 64, "
                  "or PINNJET_TC=0)"),
         "tensor_products_per_fp32_product": 6 if tc_fwd else 0,
         "fp32_ffma_peak": fp32_peak, "frac_of_fp32_ffma_peak": ach_k1 / fp32_peak,

@@ -1,7 +1,7 @@
 """Heat equation u_t = 0.3 u_xx on [0, 1] with u(0, t) given and an insulated right end, u_x(1, t) = 0: the Neumann datum
 makes ``IBVP1D`` evaluate the network AT x = 1 (reference conditions.py:585-596, 670-676); the fused engine runs that as a
 second instance of the same network sharing its weights.  Trained with the 'h1'-free default loss and optim.FlatAdam.
-python examples/heat_neumann.py   (needs a B200 and the built library)"""
+python examples/heat_neumann.py   (needs an H100 and the built library)"""
 import numpy as np
 import torch
 

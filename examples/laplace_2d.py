@@ -1,5 +1,5 @@
 """Laplace's equation on the unit square -- the reference's README example (README.md:108-130 of NeuroDiffGym/neurodiffeq)
-with the import root changed to ``neurodiffeq_b200``.  Needs a B200 (sm_100a) and the built library
+with the import root changed to ``neurodiffeq_b200``.  Needs an H100 (sm_90a) and the built library
 (``python neurodiffeq_b200/csrc/build.py``).   python examples/laplace_2d.py"""
 import numpy as np
 import torch

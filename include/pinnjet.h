@@ -1,5 +1,5 @@
 /*
- * pinnjet.h -- C ABI of libpinnjet.so: the B200-native PINN residual + parameter-gradient engine.
+ * pinnjet.h -- C ABI of libpinnjet.so: the H100-native PINN residual + parameter-gradient engine.
  *
  * The reference (NeuroDiffGym/neurodiffeq @ 9f6d6e3) has NO FFI: its hot path is the Python closure at
  * neurodiffeq/solvers.py:369-395 orchestrating ~500 ATen calls per batch.  This header is the boundary a maintainer
@@ -145,7 +145,7 @@ int pj_backward(const PjSpec* spec, const float* const* coords, int64_t n_points
                 float* grad_theta /*device, accumulated*/, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- data parallelism (SURVEY.md 8e): the one collective of the path -------------------------------------------------
- * Replaces nothing in the reference (single process); replaces the NCCL all-reduce of round 1.  Every rank passes the device
+ * Replaces nothing in the reference (single process); replaces the NCCL all-reduce of the flat gradient buffer.  Every rank passes the device
  * addresses of ONE symmetric buffer per rank (pj_allreduce_bytes(n) bytes each, zero-initialised before the first call,
  * peer-mapped on every GPU of the node: e.g. torch.distributed._symmetric_memory), its rank, and the flat float buffer
  * [grad_theta | sum r^2]; out (may alias in) receives the sum over the ranks, bit-identical on every rank.  One launch, no

@@ -1,4 +1,4 @@
-"""Build libpinnjet.so in-tree with nvcc for sm_100a (no torch involved: the library is plain C ABI + CUDA runtime).
+"""Build libpinnjet.so in-tree with nvcc for sm_90a (H100) (no torch involved: the library is plain C ABI + CUDA runtime).
 
 One object per jet-channel scheme so that the instantiations compile in parallel.  Used by __graft_entry__.build().
 """
@@ -10,7 +10,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 SCHEMES = [(1, 0, 0), (1, 1, 0), (2, 0, 0), (2, 1, 0), (2, 2, 0), (3, 0, 0), (3, 3, 0), (2, 1, 2), (3, 1, 3), (4, 1, 4)]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC",
+FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 LIB = os.path.join(HERE, "libpinnjet.so")
 LIB_TIMING = os.path.join(HERE, "libpinnjet_timing.so")   # diagnostic build with per-phase clock64 counters
@@ -59,7 +59,7 @@ def build(force=False, verbose=False, extra_flags=(), lib=None, objdir_name="bui
     with open(os.path.join(objdir, "ptxas.log"), "w") as f:
         for out, log in logs:
             f.write(f"==== {os.path.basename(out)}\n{log}\n")
-    cmd = [NVCC, "-shared", "-o", lib] + [j[0] for j in jobs] + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [NVCC, "-shared", "-o", lib] + [j[0] for j in jobs] + ["-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout + r.stderr)

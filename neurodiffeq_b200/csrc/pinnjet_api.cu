@@ -70,13 +70,16 @@ static const SchemeEntry* find_scheme(int n1, int n2, int wl) {
 static int round_up(int v, int m) { return (v + m - 1) / m * m; }
 static long long round_up_ll(long long v, long long m) { return (v + m - 1) / m * m; }
 
-constexpr int SMEM_LIMIT = 232448;   // 227 KB opt-in maximum per CTA on sm_100
+constexpr int SMEM_LIMIT = 232448;   // 227 KB opt-in maximum per CTA on sm_90
 constexpr int LOSS_PART_BYTES = 4096;
 constexpr int PROG_MAX = 1024;
 constexpr int TC_STAGE = 16 * 32 * 20 * 4;   // pinnjet_tc.cuh: TC_STAGE_BYTES
 constexpr int TC_PROG_RESERVE = 8192;   // shared-memory bytes the tensor-core plan sets aside for the programs
 #ifndef PJ_TC_DEFAULT
-#define PJ_TC_DEFAULT 2   // PINNJET_TC when the variable is unset: tensor-core forward and reverse kernels where eligible
+// PINNJET_TC when the variable is unset: the FFMA kernels.  On the H100 they are faster than the wgmma kernels for every
+// BASELINE workload the wgmma kernels can take (DESIGN.md §5: C2 0.242 vs 0.364 ms/step, C4 0.518 vs 1.095, C5 0.553 vs
+// 0.776); PINNJET_TC=1 / 2 select the tensor-core forward / forward and reverse kernels.
+#define PJ_TC_DEFAULT 0
 #endif
 
 // Weight-ring depth: keep all chunks resident if that still allows `target_occ` CTAs per SM; otherwise stream with as many
@@ -141,7 +144,7 @@ static int make_plan_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w
     if ((pl.T / pl.P) % 8 != 0 || pl.T > pl.ntc) return fail(-3, "internal: tile %d unsupported", pl.T);
     pl.RS = C * pl.T + ROW_PAD;
     pl.n_tiles = (int)((N + pl.T - 1) / pl.T);
-    // K1: 8 units per thread (half the shared-memory wavefronts per FFMA2 of the 4-unit tile); its tile is a multiple of T
+    // K1: 8 units per thread (half the shared-memory wavefronts per FFMA of the 4-unit tile); its tile is a multiple of T
     pl.ntc1 = hmax <= 64 ? 128 : 256;
     pl.P1 = C <= 2 ? 4 : 2;
     pl.Q1 = hmax > 64 ? 8 : 4;   // wide nets are GEMM-bound (fewer smem wavefronts); narrow ones want more CTAs per SM
@@ -227,7 +230,7 @@ static int make_plan_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w
         const int k2_small = round_up((sp.n_nets * PJ_MAX_NETS * 64 + 2 * (sp.n_yrows + nw_ + sp.n_coords) * tp_) * 4, 128);
         const int k2_need = 2 * 3 * 128 * 128 + TC_STAGE + tc_nhh * 3 * 64 * 128 + k2_small + rec_b +
                             round_up(4 * pl.sgrad_floats * 4, 128) + 256;
-        ok = ok && k1_need <= SMEM_LIMIT && (level < 2 || (k2_need <= SMEM_LIMIT && tc_nhh <= 7));
+        ok = ok && k1_need <= SMEM_LIMIT && (level < 2 || k2_need <= SMEM_LIMIT);
         if (ok) {
             const int CP = C <= 2 ? 2 : (C <= 4 ? 4 : 8);
             pl.tc = 1;
@@ -328,7 +331,7 @@ static int make_plan_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w
         pl.k2_small = o;   // last-Linear rows [net][4][64], then the double-buffered tile info (seeds | weights | coordinates)
         o += round_up((sp.n_nets * PJ_MAX_NETS * 64 + 2 * (sp.n_yrows + sp.n_nets * sp.wl + sp.n_coords) * pl.tp) * 4, 128);
         pl.k2_ybar = o; o += 512 * C * (pl.tp / 8) * 4;             // record block (bulk-TMA destination, 16-byte aligned)
-        pl.k2_sgrad = o; o += round_up(4 * pl.sgrad_floats * 4, 128);   // one copy per TMEM lane quarter
+        pl.k2_sgrad = o; o += round_up(4 * pl.sgrad_floats * 4, 128);   // one copy per row quarter
         pl.k2_misc = o; o += misc_bytes;
         pl.k2_bytes = o;
         pl.n_stage_bwd = 1;

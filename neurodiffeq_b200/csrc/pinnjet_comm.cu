@@ -1,8 +1,7 @@
 // pinnjet_comm.cu -- the one collective of the data-parallel path (SURVEY.md §8e): SUM of the flat [grad_theta | sum r^2]
 // buffer over the ranks of one node, as ONE kernel over NVLink peer memory.
 //
-// NCCL's all-reduce of this 34 KB message is latency bound (measured round 1: +20 / +40 / +52 us at 2 / 4 / 8 GPUs, on the
-// critical path of every step).  Here every rank owns a SYMMETRIC buffer (same layout on every GPU, peer-mapped; the host
+// NCCL's all-reduce of this 34 KB message is latency bound (tens of microseconds on the critical path of every step).  Here every rank owns a SYMMETRIC buffer (same layout on every GPU, peer-mapped; the host
 // side obtains the peer pointers once, e.g. from torch symmetric memory):
 //       [flags: PJ_AR_BLOCKS x PJ_AR_MAX_RANKS x u32][epochs: PJ_AR_BLOCKS x u32][data: 2 x n_pad floats]
 // and a call is one launch of PJ_AR_BLOCKS independent CTAs.  CTA b, epoch e (its own counter, kept on the device so that a
@@ -94,8 +93,7 @@ __global__ void __launch_bounds__(256) allreduce_oneshot_kernel(const ArArgs a, 
 }
 
 // K2b and the collective in one kernel (pj_backward_allreduce), low-latency form: the stand-alone kernel above costs two
-// NVLink traversals plus two system-scope fences per call (flag over, data back: ~12 us measured at 2 GPUs, whether or not
-// K2b is merged in front of it), so this one PUSHES instead.  Every float travels as ONE 64-bit word {epoch, value}
+// NVLink traversals plus two system-scope fences per call (flag over, data back), so this one PUSHES instead.  Every float travels as ONE 64-bit word {epoch, value}
 // (a scalar 8-byte store is single-copy atomic, also over NVLink): the receiver polls the word itself, so there is no flag,
 // no fence and no barrier between the ranks -- the critical path is one one-way store.
 //   symmetric buffer:  [epochs: PJ_ARF_BLOCKS x u32 | pad to PJ_ARF_HEADER_BYTES][slot 2][src rank world][n_pad] x u64

@@ -1,4 +1,4 @@
-// pinnjet_common.cuh -- shared definitions of the sm_100a kernels (plan, PTX helpers, jet algebra, FFMA2 microkernels).
+// pinnjet_common.cuh -- shared definitions of the sm_90a kernels (plan, PTX helpers, jet algebra, FFMA microkernels).
 //
 // Kernel family (DESIGN.md has the full picture):
 //   K0  pack      theta (torch layout) -> K-major / out-major padded copies the tiles stream with bulk TMA
@@ -13,16 +13,10 @@
 #include <stdlib.h>
 #include "../../include/pinnjet.h"
 
-#ifndef PJ_USE_FFMA2
-#define PJ_USE_FFMA2 1
-#endif
-
 namespace pj {
 
-// PINNJET_PDL=1 switches programmatic dependent launch between the kernels of a step on.  Off by default: measured on B200
-// (profiles/r02/bench_c2_v6.json vs bench_c2_nopdl_v6.json, same for C5) it does not pay -- inside a CUDA graph the kernel-to-
-// kernel gaps are already ~1 us and the early-resident dependents cost more than they hide (C2 0.1121 vs 0.1099 ms/step,
-// C5 0.2266 vs 0.2204).
+// PINNJET_PDL=1 switches programmatic dependent launch between the kernels of a step on.  Off by default: inside a CUDA
+// graph the kernel-to-kernel gaps are already short, and early-resident dependents can cost more than they hide.
 inline bool pdl_enabled() {
     static const int on = [] {
         const char* e = getenv("PINNJET_PDL");
@@ -83,7 +77,7 @@ struct Plan {
     long long b_wo[PJ_MAX_NETS][PJ_MAX_LINEAR];   //                          [out_p][in_p]  (adjoint B operand)
     long long b_wimg[PJ_MAX_NETS][PJ_MAX_LINEAR];   // tensor-core path: 3 bf16 split images of W_l, K-major SWIZZLE_128B (float offset)
     long long b_woutimg[PJ_MAX_NETS];    // tensor-core path: 3 bf16 split images [16 x 64] of the output Linear (rows >= n_out zero)
-    int tc;                              // 1: K1 runs the hidden-layer and output GEMMs on tcgen05 (pinnjet_k1tc3.cuh)
+    int tc;                              // 1: K1 runs the hidden-layer and output GEMMs on wgmma (pinnjet_k1tc3.cuh)
     int tc_bwd;                          // 1: K2 too (pinnjet_k2tc2.cuh); it reads K1-TC's records in place
     int tp;                              // tensor-core tile: points per 128 GEMM rows (pinnjet_tc.cuh: TcGeo::TP)
     int seed_T;                          // tile size of the seed / combined-weight layouts K1 writes ( = tp when tc_bwd, else T)
@@ -143,7 +137,7 @@ struct K2Args {
 };
 
 // ---------------------------------------------------------------------------------------------------------------------
-// PTX helpers: mbarrier, bulk TMA (cp.async.bulk -> SASS UBLKCP), named barriers, packed FP32 FMA (FFMA2)
+// PTX helpers: mbarrier, bulk TMA (cp.async.bulk -> SASS UBLKCP), named barriers, FP32 FMA on point pairs
 // ---------------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
@@ -233,7 +227,8 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
 template <int NTC>
 __device__ __forceinline__ void bar_compute() { asm volatile("bar.sync 1, %0;" ::"n"(NTC) : "memory"); }
 
-// packed pair of fp32 in one 64-bit register pair: the operand type of fma.rn.f32x2 (SASS FFMA2)
+// packed pair of fp32 in one 64-bit register pair (point pairs of the FFMA microkernels); sm_90 has no packed fp32 FMA,
+// so ffma2 is two FFMAs
 typedef unsigned long long f2;
 __device__ __forceinline__ f2 pack2(float x, float y) {
     f2 r;
@@ -246,12 +241,8 @@ __device__ __forceinline__ float2 unpack2(f2 v) {
     return r;
 }
 __device__ __forceinline__ void ffma2(f2& d, const f2 a, const f2 b) {
-#if PJ_USE_FFMA2
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(b));
-#else
     const float2 x = unpack2(a), y = unpack2(b), z = unpack2(d);
     d = pack2(fmaf(x.x, y.x, z.x), fmaf(x.y, y.y, z.y));
-#endif
 }
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -390,7 +381,7 @@ __device__ __forceinline__ void act_backward(int act, const float (&z)[1 + N1 + 
 // register-tile GEMM: acc[q][c][p] += sum_k A[k][c][p0+p] * B[k][u0+q]
 //   A: jet buffer rows (stride RS floats), channel c at +c*T, points contiguous       (shared memory)
 //   B: weight chunk rows (stride ldb floats), output units contiguous                  (shared memory)
-// Thread tile P points x Q units x C channels; point pairs are packed for FFMA2.
+// Thread tile P points x Q units x C channels; point pairs are packed in 64-bit register pairs.
 // ---------------------------------------------------------------------------------------------------------------------
 template <int P, int Q, int C>
 __device__ __forceinline__ void gemm_rows(f2 (&acc)[Q][C][P / 2], const float* __restrict__ a_ptr, int RS, int T,

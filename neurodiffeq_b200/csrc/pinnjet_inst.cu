@@ -17,7 +17,7 @@ namespace pj {
 #if PJ_N1 < 0
 
 // K2b: grad_theta[i] += sum over CTAs of partial[cta][i].  Block = 32 parameters x 8 groups of partials (one warp per group:
-// coalesced 128-byte rows, ~19 dependent adds per thread for 148 partials); fixed summation order -> run-to-run reproducible.
+// coalesced 128-byte rows, ~17 dependent adds per thread for 132 partials); fixed summation order -> run-to-run reproducible.
 __global__ void __launch_bounds__(RED_PARAMS * RED_GROUPS) k2_reduce_kernel(const float* __restrict__ gpart, int n_parts, long long n_theta,
                                                                              float* __restrict__ grad) {
     __shared__ float red[RED_GROUPS][RED_PARAMS];

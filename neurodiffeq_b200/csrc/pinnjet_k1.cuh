@@ -6,7 +6,7 @@
 //
 // Per tile of T points a CTA keeps ALL jet channels of one hidden layer in shared memory ([unit][channel][point],
 // row stride RS) and walks the layers: the hidden->hidden contraction for the C channels is one register-tiled
-// FP32 GEMM (FFMA2, packed point pairs) whose B operand (K-major weights) is streamed by a producer warp with bulk
+// FP32 GEMM (FFMA, point pairs) whose B operand (K-major weights) is streamed by a producer warp with bulk
 // TMA through an mbarrier ring (kept resident when all layers fit).  The activation-jet rule runs on the accumulator
 // registers, results go back to shared memory in place.  The raw network-output jets of up to 256 points are
 // collected and the residual program is then interpreted with one point per thread.

@@ -1,20 +1,21 @@
-// pinnjet_k1tc3.cuh -- K1-TC: the forward kernel with every hidden-layer contraction on the 5th-gen tensor cores.
+// pinnjet_k1tc3.cuh -- K1-TC: the forward kernel with every hidden-layer contraction on the Hopper tensor cores (wgmma).
 //
 // Same contract as k1_forward_kernel (pinnjet_k1.cuh) for networks whose hidden layers are 64 wide (any 1..8 jet
 // channels).  Geometry and operand formats: pinnjet_tc.cuh.  Warp roles of a CTA (one per SM, persistent over tiles):
-//   warps 0..15  compute: layer 0 from the coordinates, TMEM -> owner layout, activation-jet rule, z-jet records for K2,
-//                bf16x3 split + A-image rows of the next GEMM;
-//   warp 16      issues the bulk-TMA loads (weight images, small parameters, programs) and every tcgen05.mma: hidden
-//                Linear = 24 MMAs (6 split products x 4 K-steps, M = 128, N = 64), output Linear = 24 MMAs with N = 16;
-//                completion through tcgen05.commit -> mbarrier;
+//   warps 0..15  compute (4 warpgroups): layer 0 from the coordinates, accumulator -> owner layout, activation-jet rule,
+//                z-jet records for K2, bf16x3 split + A-image rows of the next GEMM; each warpgroup issues the wgmmas of
+//                its 16-unit column block: hidden Linear = 48 m64n16k16 (6 split products x 4 K-steps x 2 row halves),
+//                output Linear (warpgroup 0 only) the same with the 16-row output image;
+//   warp 16      issues the bulk-TMA loads (weight images, small parameters, programs);
 //   warps 17,18  residual-program interpreters (32 points each) working on the jet table of the PREVIOUS batch while the
 //                compute warps are already in the next tiles.
 // Software pipeline: TWO tiles are in flight per CTA (slot 0: tiles 0, 2, 4, ..; slot 1: tiles 1, 3, 5, ..), each with its
-// own A images, accumulators and mbarrier pair.  The compute warps alternate between the slots, one step per visit:
-//   visit(slot) = [wait for the slot's MMA]  consume its accumulator (epilogue of hidden layer h, or output jets)
-//                 produce the A rows of the next GEMM of that slot  ->  publish  ->  go to the other slot
-// so the MMAs + commit latency of one tile run under the epilogue of the other.  Both sides (compute warps, MMA warp) walk
-// the same deterministic step sequence, hence no work queue is needed.
+// own A images and accumulator registers.  The compute warps alternate between the slots, one step per visit:
+//   visit(slot) = consume its accumulator (epilogue of hidden layer h, or output jets)
+//                 produce the A rows of the next GEMM of that slot  ->  wait for the OTHER slot's wgmmas  ->  barrier
+//                 ->  issue the slot's wgmmas (asynchronous)  ->  go to the other slot
+// so the wgmmas of one tile run under the epilogue of the other, and the wait before the barrier guarantees that no
+// warpgroup still reads A rows another warp is about to overwrite.
 //   warp 19      prefetch: coordinates of the tiles ahead (ring of 4 tile buffers) and, for the combined second-order
 //                channel, their per-point weights (weight program) -- off the compute warps' critical path.
 // The visit body exists ONCE in the code (the slot is a run-time index): the kernel is instruction-fetch sensitive.
@@ -62,14 +63,14 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
     float* xbuf = wbuf + (size_t)K1T_RING * sp.n_nets * WL * TP;
     float* wslots = reinterpret_cast<float*>(smem + pl.k1_wslots);   // value file of the weight program
     uint64_t* wfull = reinterpret_cast<uint64_t*>(smem + pl.k1_misc);   // small parameters + programs landed
-    uint64_t* wimg_full = wfull + 19;                                   // weight images landed (only the MMA warp waits)
-    uint64_t* a_ready = wfull + 1;                                      // [2] A rows of a slot written (16 warp arrivals)
-    uint64_t* mma_done = a_ready + 2;                                   // [2] accumulator of a slot complete
-    uint64_t* yfull = mma_done + 2;                                     // [2] jet table of a batch complete
+    uint64_t* wimg_full = wfull + 19;                                   // weight images landed (the compute warps wait)
+    uint64_t* yfull = wfull + 5;                                        // [2] jet table of a batch complete
     uint64_t* yempty = yfull + 2;                                       // [2] program warps done with the buffer
     uint64_t* pre_full = yempty + 2;                                    // [4] coordinates / weights of a tile prefetched
     uint64_t* pre_empty = pre_full + K1T_RING;                          // [4] the tile is finished (16 warp arrivals)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pre_empty + K1T_RING);   // (wfull + 17; + 18: trace clock; + 19: wimg_full)
+#ifdef PJ_TIMING
+    uint32_t* clock_slot = reinterpret_cast<uint32_t*>(pre_empty + K1T_RING);  // (wfull + 17; + 18: trace clock; + 19: wimg_full)
+#endif
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int my_tiles = (pl.n_tiles1 > (int)blockIdx.x) ? (pl.n_tiles1 - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
@@ -83,13 +84,11 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
     pdl_launch_dependents();
     if (tid == 0) {
 #ifdef PJ_TIMING
-        *reinterpret_cast<unsigned long long*>(tmem_slot + 2) = clock64();
+        *reinterpret_cast<unsigned long long*>(clock_slot + 2) = clock64();
 #endif
         mbar_init(wfull, 1);
         mbar_init(wimg_full, 1);
         for (int b = 0; b < 2; ++b) {
-            mbar_init(&a_ready[b], TC_NCW);
-            mbar_init(&mma_done[b], 1);
             mbar_init(&yfull[b], 1);
             mbar_init(&yempty[b], K1T_NPW);
         }
@@ -99,27 +98,19 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
         }
         fence_barrier_init();
     }
-    if (warp == 0) {   // columns [0,128): two hidden accumulators [128 x 64]; [128,160): two output accumulators [128 x 16]
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(tmem_slot)));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     // rows of padded channels (c >= C) are never written: they must read as zero in every GEMM
     if constexpr (G::CP != C)
         for (int i = tid; i < 2 * 3 * TC_AIMG / 16; i += K1T_THREADS) reinterpret_cast<uint4*>(aimg)[i] = make_uint4(0, 0, 0, 0);
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 #ifdef PJ_TIMING
-    const unsigned long long t0_ = *reinterpret_cast<volatile unsigned long long*>(tmem_slot + 2);
+    const unsigned long long t0_ = *reinterpret_cast<volatile unsigned long long*>(clock_slot + 2);
 #endif
 
-    if (warp == TC_NCW) {   // ================= TMA + MMA warp =================
-        TC_TRACE(tr, A.dbg, 200, 100, t0_, blockIdx.x == 0 && lane == 0)
+    if (warp == TC_NCW) {   // ================= TMA warp =================
         if (lane == 0) {
             pdl_wait();   // K0 (pack) has completed.  Only this thread reads theta_pack (bulk TMA); every other warp gets the
-                          // weights through shared memory + mbarriers, so barriers / TMEM / the coordinate prefetch start early
+                          // weights through shared memory + mbarriers, so barriers / the coordinate prefetch start early
             const uint32_t small_bytes = (uint32_t)((pl.small_floats * 4 + 15) / 16 * 16);
             const uint32_t prog_bytes = (uint32_t)A.prog_len * 16u, progw_bytes = WL > 0 ? (uint32_t)A.prog_w_len * 16u : 0u;
             const uint32_t w_bytes = (uint32_t)n_hh * 3u * TC_WIMG + (uint32_t)sp.n_nets * 3u * TC_WOUT;
@@ -134,46 +125,6 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
                     tma_bulk_g2s(wimg + (size_t)slot * 3 * TC_WIMG, A.pack + pl.b_wimg[n][l], 3 * TC_WIMG, wimg_full);
             for (int n = 0; n < sp.n_nets; ++n)
                 tma_bulk_g2s(woutimg + (size_t)n * 3 * TC_WOUT, A.pack + pl.b_woutimg[n], 3 * TC_WOUT, wimg_full);
-        }
-        mbar_wait(wimg_full, 0);
-        constexpr uint32_t IDESC_HID = tc_idesc(128, TC_H, false, false), IDESC_OUT = tc_idesc(128, 16, false, false);
-        // step cursors of the two slots, packed: the GEMM that follows "hidden layer h of net n of tile iter produced"
-        int it0 = 0, it1 = 1, n0 = 0, n1 = 0, h0 = 1, h1 = 1;
-        uint32_t phases = 0;
-#pragma unroll 1
-        for (int v = 0; it0 < my_tiles || it1 < my_tiles; ++v) {
-            const int s = v & 1;
-            const int iter = s ? it1 : it0;
-            if (iter >= my_tiles) continue;
-            const int n = s ? n1 : n0, h = s ? h1 : h0, L = sp.net[n].n_linear - 1;
-            mbar_wait(&a_ready[s], (phases >> s) & 1u);
-            phases ^= 1u << s;
-            tc_fence_after();
-            TC_MARK(tr, 1 | (s << 4) | (h << 5))
-            if (lane == 0) {
-                const uint64_t da0 = umma_desc_sw128(smem_u32(aimg + (size_t)s * 3 * TC_AIMG));
-                if (h < L) {
-                    int wslot = h - 1;
-                    for (int m = 0; m < n; ++m) wslot += sp.net[m].n_linear - 2;
-                    tc_mma_split6<TC_H / 16, TC_AIMG, 32, TC_WIMG, 32>(tmem_base + (uint32_t)(s * TC_H), da0,
-                        umma_desc_sw128(smem_u32(wimg + (size_t)wslot * 3 * TC_WIMG)), IDESC_HID, false);
-                } else {
-                    tc_mma_split6<TC_H / 16, TC_AIMG, 32, TC_WOUT, 32>(tmem_base + 128u + (uint32_t)(s * 16), da0,
-                        umma_desc_sw128(smem_u32(woutimg + (size_t)n * 3 * TC_WOUT)), IDESC_OUT, false);
-                }
-                tc_commit(&mma_done[s]);
-            }
-            __syncwarp();
-            TC_MARK(tr, 2 | (s << 4) | (h << 5))
-            int nh = h + 1, nn = n, nit = iter;
-            if (h >= L) {
-                nh = 1;
-                if (++nn == sp.n_nets) {
-                    nn = 0;
-                    nit += 2;
-                }
-            }
-            if (s) { h1 = nh; n1 = nn; it1 = nit; } else { h0 = nh; n0 = nn; it0 = nit; }
         }
         return;
     }
@@ -269,12 +220,30 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
 
     // ================================================ compute warps ====================================================
     const TcThread<C> th(tid);
-    const bool out_reader = th.j == 0;                           // warps 0..3: one per TMEM lane quarter
+    const bool out_reader = th.j == 0;                           // warpgroup 0 (warps 0..3): one per row quarter
     // step cursors of the two slots: produce hidden layer h (h <= L) or read the output jets (h = L + 1)
     int it0 = 0, it1 = 1, n0 = 0, n1 = 0, h0 = 1, h1 = 1;
-    uint32_t phases = 0;
+    // ONE accumulator set (this warp's 32 x 16 block of the GEMM in flight), issued on a path every warpgroup takes.
+    // Once complete, its result is moved out at once, in owner layout (`nz`) and as the values of the lane's output row
+    // (`no`), for the slot's next visit.
+    float acc[2][8];
+    int pend = -1;                  // slot whose GEMM result is in acc (-1: none)
+    float nz[C][UG], no[PJ_MAX_NETS];
+    auto take = [&]() {             // the GEMM in acc has been waited for
+        const float* st = tc_stage_acc(acc, stage, warp, lane);
+        tc_read_owner<C>(st, th, nz);
+        static_assert(PJ_MAX_NETS == 4, "one 16-byte row read");
+        const float4 r = *reinterpret_cast<const float4*>(st + lane * TC_STAGE_STRIDE);
+        no[0] = r.x;
+        no[1] = r.y;
+        no[2] = r.z;
+        no[3] = r.w;
+        __syncwarp();
+        pend = -1;
+    };
     TC_TRACE(tr, A.dbg, 0, 200, t0_, blockIdx.x == 0 && tid == 0)
     mbar_wait(wfull, 0);
+    mbar_wait(wimg_full, 0);
     TC_MARK(tr, 0)
 
 #pragma unroll 1
@@ -284,14 +253,14 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
         if (iter >= my_tiles) continue;
         int n = s ? n1 : n0, h = s ? h1 : h0;
         unsigned char* a_slot = aimg + (size_t)s * 3 * TC_AIMG;
-        const uint32_t tmem_hid = tmem_base + (uint32_t)(s * TC_H);
-        const uint32_t tmem_out = tmem_base + 128u + (uint32_t)(s * 16);
         TC_MARK(tr, 1 | (s << 4) | (h << 5))
 
         if (h > 1) {
-            mbar_wait(&mma_done[s], (phases >> s) & 1u);
-            phases ^= 1u << s;
-            tc_fence_after();
+            if (pend == s) {   // the other slot is finished: nobody has waited for this slot's GEMM yet
+                wg_wait<0>();
+                bar_named(11, TC_NT);   // every warpgroup's GEMM has read the slot's A rows
+                take();
+            }
             TC_MARK(tr, 2 | (s << 4) | (h << 5))
             if (h > sp.net[n].n_linear - 1) {
                 // ---- output jets of net n: row = (point, channel), n_out columns -> jet table of the batch ----
@@ -301,18 +270,13 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
                     float* yb = ycache + (size_t)(b & 1) * sp.n_yrows * K1T_EB + bslot * TP;
                     const PjNet& net = sp.net[n];
                     const int n_out = net.width[net.n_linear];
-                    uint32_t o4[4];
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];\n"
-                                 : "=r"(o4[0]), "=r"(o4[1]), "=r"(o4[2]), "=r"(o4[3])
-                                 : "r"(tmem_out + ((uint32_t)(th.q * 32) << 16)));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
                     const int row = th.q * 32 + lane, pt = row / G::CP, ch = row % G::CP;
                     if (ch < C) {
                         const float* bo = small + pl.s_bout[n];
 #pragma unroll
                         for (int o = 0; o < PJ_MAX_NETS; ++o)
                             if (o < n_out)
-                                yb[(net.yrow0 + o * C + ch) * K1T_EB + pt] = __uint_as_float(o4[o]) + (ch == 0 ? bo[o] : 0.0f);
+                                yb[(net.yrow0 + o * C + ch) * K1T_EB + pt] = no[o] + (ch == 0 ? bo[o] : 0.0f);
                     }
                     if (n == sp.n_nets - 1 && (bslot == TPB - 1 || iter == my_tiles - 1)) {   // batch complete
                         bar_named(10, 128);
@@ -365,7 +329,10 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
                 for (int c = 1; c < C; ++c) z[c][k] = c <= N1 ? dzt[(c - 1) * TC_H + u] : 0.0f;
             }
         } else {
-            tc_load_owner<C>(tmem_hid, stage, th, z);
+#pragma unroll
+            for (int c = 0; c < C; ++c)
+#pragma unroll
+                for (int k = 0; k < UG; ++k) z[c][k] = nz[c][k];
             const float* bias = small + pl.s_b[n][h - 1];
 #pragma unroll
             for (int k = 0; k < UG; ++k) z[0][k] += bias[th.ubase + k];
@@ -397,14 +364,25 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
         TC_MARK(tr, 5 | (s << 4) | (h << 5))
         tc_store_rows<C>(a_slot, TC_AIMG, th, z);
         TC_MARK(tr, 6 | (s << 4) | (h << 5))
-        tc_publish(&a_ready[s], th.lane);   // -> the MMA warp issues Linear h (hidden) or the output Linear
+        wg_wait<0>();   // the other slot's GEMM is complete: after the barrier its A rows may be rewritten
+        if (pend >= 0) take();
+        tc_publish();
+        {   // Linear h (hidden: column block th.j) or the output Linear of net n (16 columns; every warpgroup computes
+            // them, warpgroup 0 reads them): descriptors by selection, the issue itself is unconditional
+            const bool hid = h < net.n_linear - 1;
+            int wslot = h - 1;
+            for (int m = 0; m < n; ++m) wslot += sp.net[m].n_linear - 2;
+            const unsigned char* bimg = hid ? wimg + (size_t)wslot * 3 * TC_WIMG + th.j * 16 * 128 : woutimg + (size_t)n * 3 * TC_WOUT;
+            wg_mma_split6<TC_H / 16, TC_AIMG, 32, 32, 0, 0, 2>(acc, wg_desc_sw128(smem_u32(a_slot), 2048),
+                                                               wg_desc_sw128(smem_u32(bimg), 1024), hid ? TC_WIMG : TC_WOUT, false);
+            wg_commit();
+            pend = s;
+        }
         TC_MARK(tr, 7 | (s << 4) | (h << 5))
         ++h;
         if (s) { it1 = iter; n1 = n; h1 = h; } else { it0 = iter; n0 = n; h0 = h; }
     }
-    tc_fence_before();
-    bar_named(9, TC_NT);
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem_base));
+    wg_wait<0>();
 }
 
 template <int N1, int N2, int WL>

@@ -3,11 +3,11 @@
 //
 // Inputs per tile: seeds dL/d(raw output jets) and the z-jets of every hidden layer, both written by K1.
 // Per hidden layer h (from the last to the first) a CTA
-//   1. pulls the adjoint of the layer's a-jets through W^T   -- register-tiled FFMA2 GEMM, out-major weights streamed by
+//   1. pulls the adjoint of the layer's a-jets through W^T   -- register-tiled FFMA GEMM, out-major weights streamed by
 //      the producer warp with bulk TMA (same ring as K1);
 //   2. applies the reverse of the activation-jet rule (needs tanh''' / sin''') on the accumulator registers, re-creating
 //      the a-jets of the layer below from its z-jets (bulk-TMA'd from the workspace) on the way;
-//   3. accumulates the weight gradient  W_bar += z_bar (x) a_prev  over channels and points -- second FFMA2 GEMM whose
+//   3. accumulates the weight gradient  W_bar += z_bar (x) a_prev  over channels and points -- second FFMA GEMM whose
 //      4x4 output tile per thread is added into a per-CTA partial buffer (thread-owned, no atomics);
 // bias / first-layer / last-layer gradients are reduced over the point lanes with warp shuffles into shared memory.
 // K2b sums the per-CTA partials into grad_theta (+=, like autograd accumulation, solvers.py:360-362).

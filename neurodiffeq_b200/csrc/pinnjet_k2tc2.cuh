@@ -1,31 +1,34 @@
-// pinnjet_k2tc2.cuh -- K2-TC: the reverse pass (dL/dtheta) with both GEMMs of every hidden->hidden Linear on tcgen05.
+// pinnjet_k2tc2.cuh -- K2-TC: the reverse pass (dL/dtheta) with both GEMMs of every hidden->hidden Linear on wgmma.
 //
 // Same contract as k2_backward_kernel (pinnjet_k2.cuh) for the problems K1-TC handles (hidden width 64, 1..8 channels):
 // reads the seeds / z-jet records / combined-channel weights K1-TC left in the workspace (tensor-core layouts, see
 // pinnjet_tc.cuh), writes this CTA's gradient partial (K2b sums them in fixed order).
 //
-// Per 128-row tile and hidden layer h = L .. 2 (operand encodings validated by experiments/tcgen05_probe):
+// Per 128-row tile and hidden layer h = L .. 2:
 //   * z_bar_h and a_{h-1} live as bf16x3 split images [128 rows x 64 units], K-major SWIZZLE_128B (ZIMG, AIMG);
 //   * adjoint GEMM   a_bar_{h-1}[r][k] = sum_j z_bar_h[r][j] W_l[j][k]:  A = ZIMG (K-major), B = the FORWARD weight images
-//     of W_l read MN-major (no transposed copy), D = [128 x 64] fp32 in TMEM, 6 split products x 4 K-steps;
+//     of W_l read MN-major (no transposed copy), 6 split products x 4 K-steps; warpgroup j computes columns 16j..16j+15 of
+//     all 128 rows (two m64 halves, pinnjet_tc.cuh) into registers;
 //   * weight-gradient GEMM  W_bar_l[j][k] += sum_r z_bar_h[r][j] a_{h-1}[r][k]:  A = ZIMG and B = AIMG both read MN-major
-//     (contraction over the rows: +2048 B per K = 16), M = 64 accumulator [64 x 64] per Linear that stays in TMEM for ALL
-//     tiles of the CTA and is read once at the end (row j in lane j%16 + 32*(j/16)).
-// Warp roles: 16 compute warps in the owner layout of pinnjet_tc.cuh, one warp that issues all MMAs, one warp that
-// streams the z-jet record blocks (bulk TMA, one hidden layer of one tile = 512 x C*UG floats) into shared memory ahead
-// of their use.  The phases of a layer overlap through mbarriers instead of CTA barriers:
+//     (contraction over the rows: +2048 B per K = 16), warpgroup j computes the [64 x 16] block of columns 16j..; the
+//     tile's product is added to this CTA's gradient partial in global memory (L2-resident; one owner thread per element,
+//     fixed order, no atomics).
+// Warp roles: 16 compute warps (4 warpgroups) in the owner layout of pinnjet_tc.cuh that also issue the wgmmas, one warp
+// that loads the weight images, one warp that streams the z-jet record blocks (bulk TMA, one hidden layer of one tile =
+// 512 x C*UG floats) into shared memory ahead of their use.  The phases of a layer overlap through asynchronous wgmmas:
 //     ADJ(h) runs  while  the compute warps turn the record of layer h-1 into AIMG;
-//     WG(h)  runs  while  they apply the reverse activation rule to the adjoint (TMEM -> owner layout).
+//     WG(h)  runs  while  they apply the reverse activation rule to the adjoint (issued after ADJ(h) has been read, so
+//            that one accumulator set is live at a time).
 // Last Linear, first Linear and all bias gradients stay on the CUDA cores: every thread sums over its own point, the PW
 // point lanes of a warp are combined by a reduce-scatter (pinnjet_tc.cuh: tc_reduce_points) and added WITHOUT atomics to
-// the copy of the small-gradient block that belongs to the warp's TMEM quarter (a unit block has one owner warp per
+// the copy of the small-gradient block that belongs to the warp's row quarter q (a unit block has one owner warp per
 // quarter); the four copies are summed when the partial is written.
 #pragma once
 #include "pinnjet_tc.cuh"
 
 namespace pj {
 
-constexpr int K2T_THREADS = TC_NT + 64;   // 576: compute warps, MMA warp, record warp
+constexpr int K2T_THREADS = TC_NT + 64;   // 576: compute warps, weight-load warp, record warp
 #ifndef PJ_WG_FIRST
 #define PJ_WG_FIRST 0                      // first split product of the weight-gradient GEMM (0: all six, 3: the three largest)
 #endif
@@ -75,15 +78,13 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
     float* recbuf = reinterpret_cast<float*>(smem + pl.k2_ybar);  // record block of the current step
     float* sgrad = reinterpret_cast<float*>(smem + pl.k2_sgrad);  // [4 quarters][sgrad_floats]
     uint64_t* wfull = reinterpret_cast<uint64_t*>(smem + pl.k2_misc);
-    uint64_t* z_ready = wfull + 1;       // ZIMG of a layer complete          (16 warp arrivals) -> ADJ
-    uint64_t* a_ready = wfull + 2;       // AIMG of the layer below complete  (16 warp arrivals) -> WG
-    uint64_t* adj_done = wfull + 3;      // adjoint accumulator complete
-    uint64_t* wg_done = wfull + 4;       // weight-gradient MMAs have read ZIMG / AIMG
     uint64_t* rec_full = wfull + 5;      // record block landed
     uint64_t* rec_empty = wfull + 6;     // every compute warp has copied its part (16 warp arrivals)
     uint64_t* ti_full = wfull + 7;       // [2] seeds / weights / coordinates of a tile staged
     uint64_t* ti_empty = wfull + 9;      // [2] the tile is finished (16 warp arrivals)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 11);
+#ifdef PJ_TIMING
+    uint32_t* clock_slot = reinterpret_cast<uint32_t*>(wfull + 11);
+#endif
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n_tiles = pl.n_tiles1;
@@ -91,18 +92,13 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
     float* gpart = A.gpart + (size_t)blockIdx.x * sp.n_theta;
     int n_hh = 0;
     for (int n = 0; n < sp.n_nets; ++n) n_hh += sp.net[n].n_linear - 2;
-    const int tmem_cols = 64 * (1 + n_hh) <= 128 ? 128 : (64 * (1 + n_hh) <= 256 ? 256 : 512);
 
     pdl_launch_dependents();
     if (tid == 0) {
 #ifdef PJ_TIMING
-        *reinterpret_cast<unsigned long long*>(tmem_slot + 2) = clock64();
+        *reinterpret_cast<unsigned long long*>(clock_slot + 2) = clock64();
 #endif
         mbar_init(wfull, 1);
-        mbar_init(z_ready, TC_NCW);
-        mbar_init(a_ready, TC_NCW);
-        mbar_init(adj_done, 1);
-        mbar_init(wg_done, 1);
         mbar_init(rec_full, 1);
         mbar_init(rec_empty, TC_NCW);
         for (int b = 0; b < 2; ++b) {
@@ -110,15 +106,6 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
             mbar_init(&ti_empty[b], TC_NCW);
         }
         fence_barrier_init();
-    }
-    if (warp == 0) {
-        if (tmem_cols == 128)
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(smem_u32(tmem_slot)));
-        else if (tmem_cols == 256)
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(tmem_slot)));
-        else
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
     }
     for (int i = tid; i < 4 * pl.sgrad_floats; i += K2T_THREADS) sgrad[i] = 0.0f;
     if constexpr (G::CP != C)   // rows of padded channels are never written: they must read as zero in both GEMMs
@@ -133,16 +120,12 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
     }
     for (long long i = tid; i < sp.n_theta; i += K2T_THREADS) gpart[i] = 0.0f;   // parameters no network of the spec owns
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 #ifdef PJ_TIMING
-    const unsigned long long t0_ = *reinterpret_cast<volatile unsigned long long*>(tmem_slot + 2);
+    const unsigned long long t0_ = *reinterpret_cast<volatile unsigned long long*>(clock_slot + 2);
 #endif
 
-    if (warp == TC_NCW) {   // ================= MMA warp (+ the weight images) =================
-        TC_TRACE(tr, A.dbg, 250, 120, t0_, blockIdx.x == 0 && lane == 0)
+    if (warp == TC_NCW) {   // ================= weight-load warp =================
         if (lane == 0) {
             if (n_hh > 0) {
                 mbar_arrive_expect_tx(wfull, (uint32_t)n_hh * 3u * TC_WIMG);
@@ -154,46 +137,7 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
                 mbar_arrive(wfull);
             }
         }
-        mbar_wait(wfull, 0);
-        constexpr uint32_t IDESC_ADJ = tc_idesc(128, TC_H, false, true), IDESC_WG = tc_idesc(64, TC_H, true, true);
-        const uint64_t dz = umma_desc_sw128(smem_u32(zimg)), da = umma_desc_sw128(smem_u32(aimg));
-        uint32_t phz = 0, pha = 0;
-#pragma unroll 1
-        for (int iter = 0; iter < my_tiles; ++iter) {
-            int slot0 = 0;
-#pragma unroll 1
-            for (int n = 0; n < sp.n_nets; ++n) {
-                const int L = sp.net[n].n_linear - 1;
-#pragma unroll 1
-                for (int h = L; h >= 2; --h) {
-                    const int slot = slot0 + (h - 2);             // Linear l = h-1 is the (l-1)-th hidden->hidden Linear
-                    mbar_wait(z_ready, phz);
-                    phz ^= 1u;
-                    tc_fence_after();
-                    TC_MARK(tr, 1 | (h << 5))
-                    if (lane == 0) {   // D_adj[r][k] = sum_j z_bar_h[r][j] W_l[j][k]
-                        tc_mma_split6<TC_H / 16, TC_AIMG, 32, TC_WIMG, 2048>(
-                            tmem_base, dz, umma_desc_sw128(smem_u32(wimg + (size_t)slot * 3 * TC_WIMG)), IDESC_ADJ, false);
-                        tc_commit(adj_done);
-                    }
-                    __syncwarp();
-                    TC_MARK(tr, 2 | (h << 5))
-                    mbar_wait(a_ready, pha);
-                    pha ^= 1u;
-                    tc_fence_after();
-                    TC_MARK(tr, 3 | (h << 5))
-                    if (lane == 0) {   // W_bar_l[j][k] += sum_r z_bar_h[r][j] a_{h-1}[r][k]; the accumulator lives across tiles
-                        tc_mma_split6<TC_ROWS / 16, TC_AIMG, 2048, TC_AIMG, 2048, PJ_WG_FIRST>(tmem_base + 64u + (uint32_t)slot * 64u, dz, da,
-                                                                                               IDESC_WG, iter > 0);
-                        tc_commit(wg_done);
-                    }
-                    __syncwarp();
-                    TC_MARK(tr, 4 | (h << 5))
-                }
-                slot0 += L - 1;
-            }
-        }
-        return;   // the compute warps read the weight-gradient accumulators after their last wg_done wait
+        return;
     }
 
     if (warp == TC_NCW + 1) {   // ================= record warp: one block per (tile, net, hidden layer), in the order of use ====
@@ -250,9 +194,13 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
     float* sg = sgrad + (size_t)th.q * pl.sgrad_floats;           // this quarter's copy of the small-gradient block
     const bool adder = (th.pt & 1) == 0;                          // after tc_reduce_points: the lane that adds value pt >> 1
     const int uadd = th.ubase + (th.pt >> 1);                     // ... which belongs to this unit
-    uint32_t ph_adj = 0, ph_wg = 0, ph_rec = 0;
-    bool wg_pending = false;             // a WG commit this thread has not waited for yet (ZIMG / AIMG still being read)
+    uint32_t ph_rec = 0;
+    float acc_adj[2][8], acc_wg[1][8];   // adjoint block (this warp's 32 x 16) / weight-gradient block of the warpgroup
+    const uint64_t dz = wg_desc_sw128(smem_u32(zimg), 2048);                    // ZIMG as the 128-row A of ADJ
+    const uint64_t dzt = wg_desc_sw128(smem_u32(zimg), 1024);                   // ZIMG as the MN-major A of WG
+    const uint64_t dat = wg_desc_sw128(smem_u32(aimg + th.j * 32), 1024);       // AIMG columns 16j.. as the B of WG
     TC_TRACE(tr, A.dbg, 0, 250, t0_, blockIdx.x == 0 && tid == 0)
+    mbar_wait(wfull, 0);
     float zr[C][UG];
 #ifdef PJ_DBG_REC_GLOBAL
     long long dbg_rec_off = 0;
@@ -365,19 +313,22 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
             }
             TC_MARK(tr, 3)
 
-            // (2) hidden layers h = L .. 2
-            if (L >= 2) {
-                if (wg_pending) {        // ZIMG / AIMG are free once the previous weight-gradient MMAs have read them
-                    mbar_wait(wg_done, ph_wg);
-                    ph_wg ^= 1u;
-                    wg_pending = false;
-                }
-                tc_store_rows<C>(zimg, TC_AIMG, th, zb);           // z_bar_L
-                tc_publish(z_ready, th.lane);                      // -> ADJ(L)
-            }
+            // (2) hidden layers h = L .. 2.  adj(h) issues ADJ(h) after z_bar_h is in ZIMG; every warpgroup has waited
+            // for its previous GEMMs, so after the barrier ZIMG / AIMG may be rewritten.
+            int slot0 = 0;
+            for (int m = 0; m < n; ++m) slot0 += sp.net[m].n_linear - 2;
+            auto adj = [&](int h) {
+                bar_named(11, TC_NT);                              // the previous GEMMs of every warpgroup have read ZIMG
+                tc_store_rows<C>(zimg, TC_AIMG, th, zb);           // z_bar_h
+                tc_publish();
+                const uint64_t dw = wg_desc_sw128(smem_u32(wimg + (size_t)(slot0 + h - 2) * 3 * TC_WIMG + th.j * 32), 1024);
+                wg_mma_split6<TC_H / 16, TC_AIMG, 32, 2048, 0, 1, 2>(acc_adj, dz, dw, TC_WIMG, false);
+                wg_commit();
+            };
             TC_MARK(tr, 4)
 #pragma unroll 1
             for (int h = L; h >= 2; --h) {
+                adj(h);                                            // z_bar_h -> ADJ(h)
                 // a_{h-1} from the record (independent of the adjoint) -> AIMG, then the weight-gradient MMAs
 #ifdef PJ_DBG_REC_GLOBAL
                 dbg_rec_off -= pl.tc_rec_layer_floats;
@@ -396,16 +347,17 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
                     }
                     tc_store_rows<C>(aimg, TC_AIMG, th, av);
                 }
-                tc_publish(a_ready, th.lane);                      // -> WG(h) (after ADJ(h) in the tensor pipe)
+                tc_publish();
                 TC_MARK(tr, 5 | (h << 5))
 
-                // adjoint of hidden h-1: TMEM -> owner layout, reverse activation rule
-                mbar_wait(adj_done, ph_adj);
-                ph_adj ^= 1u;
-                tc_fence_after();
+                // adjoint of hidden h-1: accumulator -> owner layout, then WG(h) (issued only now, so that one
+                // accumulator set is live at a time), then the reverse activation rule while WG(h) runs
+                wg_wait<0>();                                      // ADJ(h) complete
                 TC_MARK(tr, 6 | (h << 5))
                 float ab[C][UG];
-                tc_load_owner<C>(tmem_base, stage, th, ab);
+                tc_load_owner<C>(acc_adj, stage, th, ab);
+                wg_mma_split6<TC_ROWS / 16, TC_AIMG, 2048, 2048, 1, 1, 1, PJ_WG_FIRST>(acc_wg, dzt, dat, TC_AIMG, false);
+                wg_commit();
                 TC_MARK(tr, 7 | (h << 5))
                 float gbv[UG];
 #pragma unroll
@@ -426,16 +378,21 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
                     if (adder) sg[pl.g_b[n][h - 2] + uadd] += s;
                 }
                 TC_MARK(tr, 8 | (h << 5))
-                wg_pending = true;
-                if (h > 2) {             // ZIMG is rewritten: the weight-gradient MMAs of this layer must have read it
-                    mbar_wait(wg_done, ph_wg);
-                    ph_wg ^= 1u;
-                    wg_pending = false;
-                    TC_MARK(tr, 9 | (h << 5))
-                    tc_store_rows<C>(zimg, TC_AIMG, th, zb);       // z_bar_{h-1}
-                    tc_publish(z_ready, th.lane);
-                    TC_MARK(tr, 10 | (h << 5))
+                wg_wait<0>();                                      // WG(h) complete: add this tile's block
+                {   // W_bar of Linear h-1 = [width[h]][width[h-1]]; instances sharing the module add to the same words
+                    const int wj = net.width[h], wk = net.width[h - 1];
+                    float* gw = gpart + net.w_off[h - 1];
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+#pragma unroll
+                        for (int nb = 0; nb < 2; ++nb)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int jr = 16 * th.q + 8 * i + (lane >> 2), k = 16 * th.j + 8 * nb + 2 * (lane & 3) + e;
+                                if (jr < wj && k < wk) gw[jr * wk + k] += acc_wg[0][4 * nb + 2 * i + e];
+                            }
                 }
+                TC_MARK(tr, 9 | (h << 5))
             }
 
             // (3) Linear 0: W_0 gradient from z_bar_1, the coordinates and the direction vectors
@@ -463,19 +420,12 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
         if (lane == 0) mbar_arrive(&ti_empty[iter & 1]);           // the tile-info buffer may be refilled
     }
     TC_MARK(tr, 12)
-    if (wg_pending) {
-        mbar_wait(wg_done, ph_wg);
-        ph_wg ^= 1u;
-    }
-    TC_MARK(tr, 14)
 
-    // ---- this CTA's partial: small gradients (sum of the four quarter copies) from shared memory, hidden->hidden weight
-    // gradients from TMEM.  Instances of one module (boundary instances, pinnjet.h) share w_off / b_off: a later instance
-    // adds to what the first one stored. ----
-    tc_fence_after();
+    // ---- this CTA's partial: small gradients (sum of the four quarter copies) from shared memory (the hidden->hidden
+    // weight gradients are already in place).  Instances of one module (boundary instances, pinnjet.h) share w_off / b_off:
+    // a later instance adds to what the first one stored. ----
     {
         const int SG = pl.sgrad_floats;
-        int slot = 0;
 #pragma unroll 1
         for (int n = 0; n < sp.n_nets; ++n) {
             bar_named(9, TC_NT);                                   // shared-memory sums complete / previous net's stores done
@@ -504,41 +454,9 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
 #pragma unroll 1
             for (int e = tid; e < n_out; e += TC_NT) put(net.b_off[L] + e, pl.g_bout[n] + e);
             TC_MARK(tr, 16)
-#pragma unroll 1
-            for (int l = 1; l < L; ++l, ++slot) {   // M = 64 accumulator: row j in lane (j % 16) + 32 * (j / 16)
-                const int width_j = net.width[l + 1], width_k = net.width[l];
-                uint32_t v[16];
-                const uint32_t addr = tmem_base + 64u + (uint32_t)slot * 64u + (uint32_t)(th.j * 16) + ((uint32_t)(th.q * 32) << 16);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                    "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                      "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                    : "r"(addr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                const int jr = 16 * th.q + lane, k0 = th.j * 16;
-                if (lane < 16 && jr < width_j) {
-                    float* gw = gpart + net.w_off[l] + (size_t)jr * width_k + k0;
-#pragma unroll
-                    for (int i = 0; i < 16; ++i)
-                        if (k0 + i < width_k) {
-                            if (shared_w) gw[i] += __uint_as_float(v[i]); else gw[i] = __uint_as_float(v[i]);
-                        }
-                }
-            }
         }
     }
     TC_MARK(tr, 13)
-    tc_fence_before();
-    bar_named(9, TC_NT);
-    if (warp == 0) {
-        if (tmem_cols == 128)
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tmem_base));
-        else if (tmem_cols == 256)
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem_base));
-        else
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base));
-    }
 }
 
 }  // namespace pj

@@ -88,9 +88,9 @@ __device__ __forceinline__ float run_program(const int4* __restrict__ prog, int 
 
 // One out-of-line copy for the kernels that call the interpreter from several roles (code size: the tensor-core forward
 // kernel is instruction-fetch sensitive).  The arguments travel in registers (a ProgIO passed by reference would live in
-// local memory).  Measured (profiles/r02/trace_k1tc3_*): a lone warp needs ~250 cycles per interpreted instruction whatever
-// the decode looks like (three variants tried: indexed branch, branch-free selects, pre-multiplied indices) -- it issues
-// ~55 dependent SASS instructions per step at ~4.5 cycles each; only compiling the program removes that.
+// local memory).  Each interpreted instruction is a chain of some tens of dependent SASS instructions (decode, two operand
+// loads from the value file, the operation, the store) whatever the decode looks like; only compiling the program
+// (jit.py) removes that.
 static __device__ __noinline__ float run_program_rt(const int4* prog, int len, float* slot,
                                                     const float* const* coords, long long gidx, long long N,
                                                     const float* ycache, int ystride, const float* rbar, float loss_scale,

@@ -1,20 +1,22 @@
-// pinnjet_tc.cuh -- shared pieces of the tcgen05 kernels (K1-TC forward, K2-TC reverse): tile geometry, bf16x3 split
-// images, the TMEM -> owner-layout transposition, MMA issue helpers.
+// pinnjet_tc.cuh -- shared pieces of the wgmma kernels (K1-TC forward, K2-TC reverse): tile geometry, bf16x3 split
+// images, the accumulator -> owner-layout transposition, wgmma issue helpers.
 //
 // GEMM formulation (hidden width 64, C jet channels padded to CP in {2, 4, 8}):
 //   * a tile is 128 GEMM rows r = CP*p + c  (point p < TP = 128/CP, channel c < C; rows with c >= C stay zero);
 //   * operands are split into THREE bf16 terms (x = x1 + x2 + x3) stored as K-major SWIZZLE_128B shared-memory images
 //     [rows x 64 units]; the six products whose weight is >= 2^-24 reproduce the fp32 contraction to ~5e-7;
-//   * accumulators are fp32 in TMEM; row r of an M = 128 accumulator is TMEM lane r.
-// Thread geometry of BOTH kernels (16 compute warps = 512 threads per tile):
-//   warp w:  q = w & 3 (TMEM lane quarter = rows 32q..32q+31), j = w >> 2 (units 16j..16j+15);
+//   * accumulators are fp32 registers of the warpgroup that issues the wgmma.
+// Thread geometry of BOTH kernels (16 compute warps = 4 warpgroups = 512 threads per tile):
+//   warp w:  q = w & 3 (rows 32q..32q+31; the warp's rank inside its warpgroup), j = w >> 2 (units 16j..16j+15; the
+//            warpgroup);
 //   lane l:  pt = l / NUG, ug = l % NUG   (NUG = 16 / UG unit groups per 16-unit block);
 //   the thread OWNS point p = q*PW + pt and the UG adjacent units ubase = 16*j + UG*ug .. of it, all channels.
-// A warp reads its 32 x 16 accumulator block from TMEM (one tcgen05.ld.32x32b.x16, lane = row), parks it in its private
-// staging block and reads it back in owner layout (only __syncwarp in between): tanh once per (point, unit), no
-// shuffles in the jet rules.  Because both kernels use the same map, the z-jet records K1 leaves for K2 are simply
-// indexed by thread:  record(tile, layer)[tid][c][k], C*UG contiguous floats per thread (64 B for C = 4): coalesced
-// 16-byte accesses.
+// Warpgroup j computes the [128 x 16] column block j of a [128 x 64] product as two m64n16 wgmmas whose A descriptors
+// take every other 8-row group (SBO = 2048 B, the second one starts 1024 B later): warp q of the warpgroup then holds
+// exactly rows 32q..32q+31 of the block -- its own 32 x 16 owner block.  It parks the fragment in its private staging
+// block and reads it back in owner layout (only __syncwarp in between): tanh once per (point, unit), no shuffles in the
+// jet rules.  Because both kernels use the same map, the z-jet records K1 leaves for K2 are simply indexed by thread:
+// record(tile, layer)[tid][c][k], C*UG contiguous floats per thread (64 B for C = 4): coalesced 16-byte accesses.
 #pragma once
 #include "pinnjet_common.cuh"
 
@@ -27,7 +29,9 @@ constexpr int TC_WIMG = TC_H * 128;      // bytes of one split image of a hidden
 constexpr int TC_WOUT = 16 * 128;        // bytes of one split image of an output layer (16 rows: outputs, zero padded)
 constexpr int TC_NCW = 16;               // compute warps
 constexpr int TC_NT = TC_NCW * 32;       // compute threads
-constexpr int TC_STAGE_STRIDE = 20;      // floats per staged TMEM row (16 + 4: conflict-free 16-byte accesses)
+constexpr int TC_STAGE_STRIDE = 20;      // floats per staged accumulator row (16 + 4): row reads (16 B per lane) are
+                                         // conflict-free, fragment stores and owner-layout reads at most 2-way
+                                         // (tests/test_tc_layout.py)
 constexpr int TC_STAGE_BYTES = TC_NCW * 32 * TC_STAGE_STRIDE * 4;   // one private 32 x 16 block per compute warp
 
 template <int C>
@@ -40,9 +44,10 @@ struct TcGeo {
     static constexpr int REC = C * UG;                         // record floats per thread and hidden layer
 };
 
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-    // 128-byte swizzle, 8-row groups 1024 B apart (SBO), descriptor version 1 (validated by experiments/tcgen05_probe)
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)64 << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+// wgmma shared-memory matrix descriptor, 128-byte swizzle (layout type 1 in bits 62-63).  `sbo`: bytes between 8-row
+// groups (K-major: along M/N; MN-major: along K).  The leading byte offset is unused by the layouts of these kernels.
+__device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t saddr, uint32_t sbo) {
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(sbo >> 4) << 32) | ((uint64_t)1 << 62);
 }
 __device__ __forceinline__ uint32_t sw128_off(int row, int chunk16) {   // byte offset of 16-byte chunk `chunk16` of `row`
     return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk16 ^ (row & 7)) << 4));
@@ -66,40 +71,41 @@ __device__ __forceinline__ void split3_bf16(float x0, float x1, uint32_t& t1, ui
 __device__ __forceinline__ void bar_named(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// instruction descriptor of tcgen05.mma.kind::f16: fp32 accumulator, bf16 A and B; optional MN-major operands
-__host__ __device__ constexpr uint32_t tc_idesc(int M, int N, bool a_mn, bool b_mn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn ? (1u << 15) : 0u) | (b_mn ? (1u << 16) : 0u) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void tc_mma(uint32_t d_tmem, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+// one m64n16k16 wgmma, bf16 operands from shared memory, fp32 accumulator d[8] (d = A B + (acc ? d : 0));
+// TA / TB = 1: the operand is MN-major
+template <int TA, int TB>
+__device__ __forceinline__ void wg_mma_m64n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// the six split products over KSTEPS K = 16 steps, SMALLEST FIRST (a1 b3, a3 b1, a2 b2, a1 b2, a2 b1, a1 b1): the tensor core
-// truncates when it adds into the fp32 accumulator, an error proportional to the accumulator's magnitude at that moment --
-// only the last KSTEPS MMAs run at full magnitude (measured on C4: rms error 5.5e-7 -> see DESIGN.md).  `da0` / `db0` are the
-// descriptors of term 0, K-step 0; the other 23 differ only in the start-address field (bytes >> 4), so every MMA costs
-// two 64-bit adds with immediates.
+// The six split products over KSTEPS K = 16 steps, SMALLEST FIRST (a1 b3, a3 b1, a2 b2, a1 b2, a2 b1, a1 b1): the tensor
+// core truncates when it adds into the fp32 accumulator, an error proportional to the accumulator's magnitude at that
+// moment -- only the last KSTEPS MMAs run at full magnitude.  `da0` / `db0` are the descriptors of term 0, K-step 0; the
+// others differ only in the start-address field (bytes >> 4); `b_img` is the byte distance of the B terms.  NA = 2: the A operand is the 128-row tile, issued as two
+// m64 halves (every other 8-row group, see the header) into d[0] / d[1]; NA = 1: one m64 product into d[0].
 // FIRST = 3 issues only the three largest products (a1 b2, a2 b1, a1 b1): ~2^-17 relative instead of ~2^-24.
-template <int KSTEPS, uint32_t A_IMG, uint32_t A_KSTEP, uint32_t B_IMG, uint32_t B_KSTEP, int FIRST = 0>
-__device__ __forceinline__ void tc_mma_split6(uint32_t d_tmem, uint64_t da0, uint64_t db0, uint32_t idesc, bool accumulate_first) {
+// Issued by a whole warpgroup; the caller commits and waits.
+template <int KSTEPS, uint32_t A_IMG, uint32_t A_KSTEP, uint32_t B_KSTEP, int TA, int TB, int NA, int FIRST = 0>
+__device__ __forceinline__ void wg_mma_split6(float (&d)[NA][8], uint64_t da0, uint64_t db0, uint32_t b_img, bool accumulate_first) {
+    wg_fence();
 #pragma unroll
     for (int pr = FIRST; pr < 6; ++pr)
 #pragma unroll
         for (int k = 0; k < KSTEPS; ++k) {
-            constexpr int TA[6] = {0, 2, 1, 0, 1, 0}, TB[6] = {2, 0, 1, 1, 0, 0};
-            const uint64_t da = da0 + (uint64_t)((TA[pr] * A_IMG + k * A_KSTEP) >> 4);
-            const uint64_t db = db0 + (uint64_t)((TB[pr] * B_IMG + k * B_KSTEP) >> 4);
-            tc_mma(d_tmem, da, db, idesc, (accumulate_first || pr > FIRST || k) ? 1u : 0u);
+            constexpr int TA_[6] = {0, 2, 1, 0, 1, 0}, TB_[6] = {2, 0, 1, 1, 0, 0};
+            const uint64_t da = da0 + (uint64_t)((TA_[pr] * A_IMG + k * A_KSTEP) >> 4);
+            const uint64_t db = db0 + (uint64_t)((TB_[pr] * b_img + k * B_KSTEP) >> 4);
+            const uint32_t acc = (accumulate_first || pr > FIRST || k) ? 1u : 0u;
+            wg_mma_m64n16<TA, TB>(d[0], da, db, acc);
+            if constexpr (NA == 2) wg_mma_m64n16<TA, TB>(d[NA - 1], da + (1024u >> 4), db, acc);
         }
 }
 
@@ -181,31 +187,28 @@ __device__ __forceinline__ void tc_store_rows(unsigned char* img, uint32_t img_b
     }
 }
 
-// TMEM accumulator block (rows 32q.., units 16j..) -> owner layout through the warp's private staging block.  `tmem_acc`:
-// TMEM address of column 0 / lane 0 of the accumulator.  The caller has waited for the MMA (mbarrier) and issued
-// tcgen05.fence::after_thread_sync.
+// The warp's 32 x 16 accumulator block (two m64n16 halves, see the header) -> its private staging block, row-major with
+// TC_STAGE_STRIDE floats per row.  Half h, register 4*nb + 2*i + e holds row 16*i + 8*h + lane/4, column
+// 8*nb + 2*(lane%4) + e.  The caller has waited for the wgmma.
+__device__ __forceinline__ float* tc_stage_acc(const float (&d)[2][8], float* stage, int warp, int lane) {
+    float* my_stage = stage + (size_t)warp * 32 * TC_STAGE_STRIDE;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int nb = 0; nb < 2; ++nb)
+                *reinterpret_cast<float2*>(my_stage + (16 * i + 8 * h + (lane >> 2)) * TC_STAGE_STRIDE + 8 * nb + 2 * (lane & 3)) =
+                    make_float2(d[h][4 * nb + 2 * i], d[h][4 * nb + 2 * i + 1]);
+    __syncwarp();
+    return my_stage;
+}
+
+// the staged block (tc_stage_acc) read back in owner layout: rows CP*pt + c, units UG*ug ..
 template <int C>
-__device__ __forceinline__ void tc_load_owner(uint32_t tmem_acc, float* stage, const TcThread<C>& t,
-                                              float (&v)[C][TcGeo<C>::UG]) {
+__device__ __forceinline__ void tc_read_owner(const float* my_stage, const TcThread<C>& t, float (&v)[C][TcGeo<C>::UG]) {
     using G = TcGeo<C>;
     constexpr int UG = G::UG;
-    float* my_stage = stage + (size_t)t.warp * 32 * TC_STAGE_STRIDE;
-    {
-        uint32_t r[16];
-        const uint32_t addr = tmem_acc + (uint32_t)(t.j * 16) + ((uint32_t)(t.q * 32) << 16);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-            : "r"(addr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        float* dst = my_stage + t.lane * TC_STAGE_STRIDE;
-#pragma unroll
-        for (int s = 0; s < 4; ++s)
-            *reinterpret_cast<uint4*>(dst + 4 * s) = make_uint4(r[4 * s], r[4 * s + 1], r[4 * s + 2], r[4 * s + 3]);
-    }
-    __syncwarp();
     const float* src = my_stage + (size_t)(G::CP * t.pt) * TC_STAGE_STRIDE + t.ug * UG;
 #pragma unroll
     for (int c = 0; c < C; ++c) {
@@ -224,16 +227,21 @@ __device__ __forceinline__ void tc_load_owner(uint32_t tmem_acc, float* stage, c
             }
         }
     }
+}
+
+// accumulator block (rows 32q.., units 16j..) -> owner layout through the warp's private staging block
+template <int C>
+__device__ __forceinline__ void tc_load_owner(const float (&d)[2][8], float* stage, const TcThread<C>& t,
+                                              float (&v)[C][TcGeo<C>::UG]) {
+    tc_read_owner<C>(tc_stage_acc(d, stage, t.warp, t.lane), t, v);
     __syncwarp();   // every lane has its values: the block may be overwritten by the next call
 }
 
-// "my part of the operand is written": make the generic-proxy stores visible to the tensor core (async proxy), then one
-// arrival per warp on an mbarrier the MMA warp waits on (count = TC_NCW)
-__device__ __forceinline__ void tc_publish(uint64_t* bar, int lane) {
+// "the operand images are written": make the generic-proxy stores visible to the tensor core (async proxy), then a
+// barrier of the 16 compute warps (every warpgroup reads rows every warp wrote)
+__device__ __forceinline__ void tc_publish() {
     fence_proxy_async();
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar);
+    bar_named(11, TC_NT);
 }
 
 // z-jet record of one hidden layer: C*UG contiguous floats per thread

@@ -27,7 +27,7 @@ class EagerProblem:
                  enforce=None, reason=""):
         if device is None:
             if not torch.cuda.is_available():
-                raise RuntimeError("the PINN engine needs a CUDA device (B200, sm_100a); none is visible")
+                raise RuntimeError("the PINN engine needs a CUDA device (H100, sm_90a); none is visible")
             device = torch.device("cuda", torch.cuda.current_device())
         self.device = torch.device(device)
         self.reason = reason

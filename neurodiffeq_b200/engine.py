@@ -61,7 +61,7 @@ def load_library():
         return _lib
     if not os.path.exists(_LIB_PATH):
         raise RuntimeError(f"{_LIB_PATH} is missing: build it with `python neurodiffeq_b200/csrc/build.py` "
-                           f"(needs nvcc, sm_100a).  There is no non-CUDA fallback for the fused path.")
+                           f"(needs nvcc, sm_90a).  There is no non-CUDA fallback for the fused path.")
     lib = ctypes.CDLL(_LIB_PATH)
     vp, i32, i64, f32 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float
     lib.pj_abi_version.restype = ctypes.c_int
@@ -165,7 +165,7 @@ class FusedProblem:
         self.lib = load_library()
         if device is None:
             if not torch.cuda.is_available():
-                raise RuntimeError("the fused PINN engine needs a CUDA device (B200, sm_100a); none is visible")
+                raise RuntimeError("the fused PINN engine needs a CUDA device (H100, sm_90a); none is visible")
             device = torch.device("cuda", torch.cuda.current_device())
         self.device = torch.device(device)
         self.tp = TracedProblem(nets, conditions, diff_eqs, n_coords, coords_for_condition, pad_scheme=pad_scheme,
@@ -663,7 +663,7 @@ class FusedProblem:
         """One WHOLE training step as a single CUDA-graph replay: zero the gradient buffer, K0..K2b on ``coords`` and the
         parameter update of a capturable :class:`neurodiffeq_b200.optim.FlatAdam` (its step is a fixed sequence of device
         operations).  Returns ``self.sumsq`` (sum of squared residuals of the step, BEFORE the update).
-        Not used by the solvers yet -- added for the fit-loop work of round 2 (DESIGN.md §9.5); single rank only."""
+        Not used by the solvers yet; single rank only."""
         if not getattr(optimizer, "capturable", False):
             raise ValueError("train_step_graphed needs FlatAdam(..., capturable=True)")
         n = coords[0].numel()

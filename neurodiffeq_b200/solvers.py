@@ -179,7 +179,7 @@ class BaseSolver:
             self.n_eq = self.problem.n_eq - (n_coords if self._h1 else 0)     # the user's equations
         self.device = self.problem.device
         # The residual programs compiled INTO the forward kernel (jit.py: ~1 s of nvcc per problem, cached on disk; identical
-        # numbers).  Default (jit=None): on whenever it applies -- tensor-core path, a compiler on the machine -- and silently
+        # numbers).  Default (jit=None): on whenever it applies -- tensor-core path (PINNJET_TC=1/2), a compiler on the machine -- and silently
         # the in-kernel interpreter otherwise (problem.jit_reason says why); jit=False or PINNJET_JIT=0 keep the interpreter.
         env = os.environ.get("PINNJET_JIT")
         if jit or (jit is None and env != "0") or (jit is not False and env == "1"):

@@ -37,8 +37,6 @@ def rel_l2(a_list, b_list):
 #   1/(r^2 sin^2 theta), up to ~6e3 on the sampled domain, so a 1-ulp error of a jet shows up as ~1e-5 in r):
 #       99.9 % of the points within 2e-5 * rms(r) + 1e-6,  max|dr| <= 1e-4 * rms(r) + 1e-6,  and the rms of the error no
 #       worse than 4x the rms error of the reference's OWN float32 run on the same inputs (``ref["residual32"]``).
-#   Measured on B200 (profiles/r01/precision_v1.log): C4 N=32768 ours max 2.2e-5 / rms-err 2.4e-7 vs reference-fp32
-#   max 1.2e-5 / rms-err 1.6e-7; C2 / C3: ours == reference-fp32 to two digits.
 TOL_RESID = 2e-5
 TOL_RESID_MAX_ILL = 1e-4
 TOL_LOSS = 1e-5       # relative

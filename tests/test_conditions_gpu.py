@@ -68,7 +68,7 @@ def test_boundary_values_are_satisfied():
 
 # ----------------------------------------------------------------------------------------------------------------------
 # EnsembleCondition (x7), IBVP1D with Neumann data on both ends through a shared jet direction (x8), Resnet (x9), 'h1 semi'
-# and function-dependent losses: confirmed on a B200 in round 2 (profiles/r02/pytest_gpu_call1.log), always on since.
+# and function-dependent losses.
 # ----------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("key", ["x7", "x8", "x9"])
 def test_later_extension_workloads_match_reference_golden(key):

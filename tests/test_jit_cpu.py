@@ -105,7 +105,7 @@ def test_module_source_names_the_scheme_and_refuses_trainable_immediates():
 
 
 @pytest.mark.skipif(not os.path.exists("/usr/local/cuda/bin/nvcc"), reason="no nvcc")
-def test_specialised_kernel_compiles_for_sm_100a(tmp_path, monkeypatch):
+def test_specialised_kernel_compiles_for_sm_90a(tmp_path, monkeypatch):
     from neurodiffeq_b200 import jit
     from neurodiffeq_b200.engine import combine_seconds
     from neurodiffeq_b200.tracing import TracedProblem

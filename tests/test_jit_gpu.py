@@ -13,6 +13,13 @@ from test_kernels_gpu import run_fused
 pytestmark = pytest.mark.gpu
 
 
+@pytest.fixture(autouse=True)
+def _tensor_core_kernels(monkeypatch):
+    """The specialised kernel is the tensor-core forward kernel with the programs compiled in: select that path (the
+    default is the FFMA kernels)."""
+    monkeypatch.setenv("PINNJET_TC", "2")
+
+
 @pytest.mark.parametrize("key,n", [("c2", 16384), ("c4", 5000), ("c5", 20011), ("x1", 3001), ("x2", 1024)])
 def test_specialised_kernel_is_identical_to_the_interpreter(key, n):
     wl, nets, conds, fp = build_fused(key, seed=21)

@@ -2,8 +2,9 @@
 tc_reduce_points; csrc/pinnjet_k1tc3.cuh / pinnjet_k2tc2.cuh), restated in numpy.
 
 A tile is 128 GEMM rows r = CP*p + c (point p, channel c, channels padded to CP in {2, 4, 8}) x 64 hidden units.  The kernels
-move such a block between three layouts: the TMEM row layout (lane = row, one tcgen05.ld.32x32b.x16 per warp = 32 rows x 16
-units), the K-major SWIZZLE_128B shared-memory images the MMAs read, and the OWNER layout of the epilogues (a thread holds
+move such a block between three layouts: the wgmma accumulator fragments (warpgroup j = column block 16j.., two m64n16
+halves over every other 8-row group, so warp q holds rows 32q.. x 16 units), the K-major SWIZZLE_128B shared-memory images
+the MMAs read, and the OWNER layout of the epilogues (a thread holds
 all channels of one point x UG adjacent units) -- which is also the layout of the z-jet records K1-TC leaves for K2-TC.
 The formulas below are the ones in the kernels; the tests pin their invariants."""
 import numpy as np
@@ -50,26 +51,82 @@ def test_owner_layout_is_a_partition_of_the_tile(C):
     assert np.all(seen == 1)                       # every (point, unit) has exactly one owner thread
 
 
+def fragment(acc, q, j, lane):
+    """Registers d[half][8] of lane `lane` of warp q in warpgroup j after wg_mma_split6<.., NA = 2>: half h reads the A rows
+    of 8-row groups 2g + h (descriptor SBO = 2048 B, start + 1024 B * h); the m64n16 accumulator layout puts register
+    4*nb + 2*i + e at m-row 16q + lane/4 + 8i, column 8nb + 2*(lane%4) + e."""
+    d = np.zeros((2, 8))
+    for h in range(2):
+        for nb in range(2):
+            for i in range(2):
+                for e in range(2):
+                    m = 16 * q + lane // 4 + 8 * i
+                    row = 8 * (2 * (m // 8) + h) + m % 8
+                    d[h, 4 * nb + 2 * i + e] = acc[row, 16 * j + 8 * nb + 2 * (lane % 4) + e]
+    return d
+
+
 @pytest.mark.parametrize("C", [2, 4, 5])
-def test_tmem_block_to_owner_layout_through_the_private_staging_block(C):
-    """tc_load_owner: warp (q, j) reads rows 32q.. x units 16j.. (lane = row), stores its 16 values at stage[lane][0:16],
-    and reads back rows CP*pt + c, columns UG*ug ..: exactly the (point, channel, unit) values it owns."""
+def test_accumulator_fragments_to_owner_layout_through_the_private_staging_block(C):
+    """tc_stage_acc + tc_load_owner: warp (q, j) stores its wgmma fragments (rows 32q.. x units 16j..) at
+    stage[16i + 8h + lane/4][8nb + 2*(lane%4) + e], and reads back rows CP*pt + c, columns UG*ug ..: exactly the
+    (point, channel, unit) values it owns."""
     g = geo(C)
     acc = np.arange(ROWS * H, dtype=np.float64).reshape(ROWS, H)      # accumulator [row][unit]
     for warp in range(NCW):
         q, j = warp & 3, (warp >> 2) & 3
         stage = np.full((32, STAGE_STRIDE), np.nan)
         for lane in range(32):
-            stage[lane, :16] = acc[32 * q + lane, 16 * j:16 * j + 16]
+            d = fragment(acc, q, j, lane)
+            for h in range(2):
+                for i in range(2):
+                    for nb in range(2):
+                        for e in range(2):
+                            r, col = 16 * i + 8 * h + lane // 4, 8 * nb + 2 * (lane % 4) + e
+                            assert np.isnan(stage[r, col])                   # every staged word written once
+                            stage[r, col] = d[h, 4 * nb + 2 * i + e]
+        np.testing.assert_array_equal(stage[:, :16], acc[32 * q:32 * q + 32, 16 * j:16 * j + 16])
         for lane in range(32):
             t = thread(C, warp * 32 + lane)
             for c in range(C):
                 got = stage[g["CP"] * t["pt"] + c, g["UG"] * t["ug"]:g["UG"] * t["ug"] + g["UG"]]
                 want = acc[t["R0"] + c, t["ubase"]:t["ubase"] + g["UG"]]
                 np.testing.assert_array_equal(got, want)
-    # conflict-free 16-byte accesses: the 8 lanes of a quarter-warp hit 8 distinct 16-byte bank groups
-    for lane0 in range(0, 32, 8):
-        assert len({((lane0 + k) * STAGE_STRIDE * 4 // 16) % 8 for k in range(8)}) == 8
+
+
+def conflict_degree(word_addrs, width):
+    """Shared-memory wavefronts per access phase for one warp instruction: lane l accesses `width` consecutive 4-byte words
+    from word_addrs[l]; a phase serves 128 bytes (32 / 16 / 8 lanes for 4 / 8 / 16-byte accesses); within a phase, distinct
+    words of one of the 32 banks are served one wavefront each."""
+    per = {1: 32, 2: 16, 4: 8}[width]
+    worst = 1
+    for p0 in range(0, 32, per):
+        banks = {}
+        for lane in range(p0, p0 + per):
+            for w in range(width):
+                a = word_addrs[lane] + w
+                banks.setdefault(a % 32, set()).add(a)
+        worst = max(worst, max(len(v) for v in banks.values()))
+    return worst
+
+
+@pytest.mark.parametrize("C", [1, 2, 3, 4, 5, 8])
+def test_staging_block_bank_conflicts(C):
+    """The accesses of the private staging block with STAGE_STRIDE = 20: the output-row read of K1 (one 16-byte load of
+    row `lane`) is conflict-free; the float2 fragment stores (tc_stage_acc) and the owner-layout reads (tc_read_owner) are
+    at most 2-way, and the owner reads are conflict-free for 3 and 4 channels."""
+    g = geo(C)
+    assert conflict_degree([lane * STAGE_STRIDE for lane in range(32)], 4) == 1
+    for h in range(2):
+        for i in range(2):
+            for nb in range(2):
+                rows = [16 * i + 8 * h + lane // 4 for lane in range(32)]
+                assert conflict_degree([r * STAGE_STRIDE + 8 * nb + 2 * (lane & 3) for lane, r in enumerate(rows)], 2) <= 2
+    UG, NUG, CP = g["UG"], g["NUG"], g["CP"]
+    for c in range(C):
+        for s4 in range(max(UG // 4, 1)):
+            addrs = [(CP * (lane // NUG) + c) * STAGE_STRIDE + (lane % NUG) * UG + 4 * s4 for lane in range(32)]
+            assert conflict_degree(addrs, min(UG, 4)) <= (1 if C in (3, 4) else 2)
 
 
 @pytest.mark.parametrize("C", [2, 3, 4, 5, 7])
