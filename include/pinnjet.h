@@ -92,7 +92,7 @@ int pj_sizes(const PjSpec* spec, int64_t n_points, PjSizes* out);
 /* Diagnostics: the tiling plan as int64 numbers (tests compare workspace contents with the CPU mirror).
  * out[0..18] = T,P,Q,C,RS,n_tiles,grid,hmax,n_stage_fwd,n_stage_bwd,resident_fwd,resident_bwd,zj_tile_floats,
  *              ws_zj,ws_seed,ws_gpart,ws_bytes,smem_fwd,smem_bwd; then hp[net][0..8] and zj_off[net][0..7] per net; then
- *              tc, tc_bwd (1: the forward / reverse kernel of this problem runs on the tensor cores), tile points of those
+ *              tc, tc_bwd (1: the forward and reverse kernels of this problem run on the tensor cores; always equal), tile points of those
  *              kernels, ws_tcrec, grid_bwd, n_tiles_fwd.  T / n_tiles describe the layout of the seeds in the workspace. */
 int pj_plan_info(const PjSpec* spec, int64_t n_points, int64_t* out, int32_t n_out);
 

@@ -17,7 +17,7 @@ LIB_TIMING = os.path.join(HERE, "libpinnjet_timing.so")   # diagnostic build wit
 
 
 def _sources():
-    return [os.path.join(HERE, f) for f in sorted(os.listdir(HERE)) if f.endswith((".cu", ".cuh", ".h"))] + \
+    return [os.path.join(HERE, f) for f in sorted(os.listdir(HERE)) if f.endswith((".cu", ".cuh", ".h", ".cpp"))] + \
         [os.path.join(HERE, "..", "..", "include", "pinnjet.h"), os.path.abspath(__file__)]
 
 
@@ -42,6 +42,7 @@ def build(force=False, verbose=False, extra_flags=(), lib=None, objdir_name="bui
     objdir = os.path.join(HERE, objdir_name)
     os.makedirs(objdir, exist_ok=True)
     jobs = [(os.path.join(objdir, "api.o"), os.path.join(HERE, "pinnjet_api.cu"), list(extra_flags)),
+            (os.path.join(objdir, "plan.o"), os.path.join(HERE, "pinnjet_plan.cpp"), list(extra_flags)),
             (os.path.join(objdir, "comm.o"), os.path.join(HERE, "pinnjet_comm.cu"), list(extra_flags)),
             (os.path.join(objdir, "sample.o"), os.path.join(HERE, "pinnjet_sample.cu"), list(extra_flags)),
             (os.path.join(objdir, "optim.o"), os.path.join(HERE, "pinnjet_optim.cu"), list(extra_flags)),

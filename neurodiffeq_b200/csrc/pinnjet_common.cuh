@@ -1,4 +1,5 @@
-// pinnjet_common.cuh -- shared definitions of the sm_90a kernels (plan, PTX helpers, jet algebra, FFMA microkernels).
+// pinnjet_common.cuh -- shared definitions of the sm_90a kernels (kernel arguments, PTX helpers, jet algebra, FFMA
+// microkernels).  The plan and its layout constants: pinnjet_plan.h.
 //
 // Kernel family (DESIGN.md has the full picture):
 //   K0  pack      theta (torch layout) -> K-major / out-major padded copies the tiles stream with bulk TMA
@@ -11,7 +12,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
-#include "../../include/pinnjet.h"
+#include "pinnjet_plan.h"
 
 namespace pj {
 
@@ -42,60 +43,16 @@ inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, 
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
-// CTA shape: NTC compute threads (128 or 256: template parameter of the kernels) + one producer warp.  Narrow networks
+// CTA shape: NTC compute threads (128 or 256: template parameter of the kernels) + service warps.  Narrow networks
 // (hidden width <= 64) use 128-thread CTAs so that several CTAs share an SM and their GEMM / activation / program phases
-// overlap; the residual program is batched over NTC points (one per compute thread).
-constexpr int CHUNK_FLOATS = 4096;       // weight chunk = 16 KB
-constexpr int MAX_STAGES = 8;
-constexpr int ROW_PAD = 4;               // jet rows are C*T + 4 floats: conflict-free row-strided float4 loads
+// overlap; the residual program is batched over NTC points (one per compute thread).  Chunk, ring and row-padding sizes:
+// pinnjet_plan.h.
 
 // opcodes of the residual program (mirror of neurodiffeq_b200/symbolic.py)
 enum : int {
     OP_CONST = 0, OP_COORD, OP_NET, OP_RBAR, OP_PARAM, OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_NEG, OP_SIN, OP_COS, OP_EXP,
     OP_LOG, OP_TANH, OP_SQRT, OP_ABS, OP_SIGN, OP_POWC, OP_RCP, OP_ST_U, OP_ST_R, OP_ST_SEED, OP_TAN, OP_SINH, OP_COSH,
     OP_ATAN, OP_ERF, OP_ST_W
-};
-
-// Everything derived from (spec, N): identical on host and device, computed by make_plan() in pinnjet_api.cu.
-struct Plan {
-    int T, P, Q, C, RS;                  // K2 tile: points, thread tile, channels, jet row stride (floats); also the
-                                         // layout of the z-jet records and seeds K1 leaves in the workspace
-    int epi_batch;                       // points per residual-program batch (jet table double-buffered in smem)
-    int T1, P1, Q1, RS1, ntc1, n_tiles1; // K1 tile (a multiple of T): wider thread tile (Q1 = 8) -> fewer smem wavefronts
-    int n_tiles, grid, grid_bwd, hmax, ntc;   // grid: K1 CTAs (= loss partials), grid_bwd: K2 CTAs (= gradient partials)
-    int n_stage, n_stage_bwd, resident_fwd, resident_bwd, chunks_fwd, chunks_bwd;   // n_stage: forward ring
-    int hp[PJ_MAX_NETS][PJ_MAX_LINEAR + 1];   // padded widths (hidden -> multiple of 32; input/output unpadded)
-    // ---- packed parameter copy (float offsets) ----
-    int small_floats;
-    int s_wt0[PJ_MAX_NETS];              // [n_in][hp1]       first Linear, K-major
-    int s_dz[PJ_MAX_NETS];               // [PJ_MAX_DIRS][hp1] first-order seeds  W0 . dir_f  (point independent)
-    int s_b[PJ_MAX_NETS][PJ_MAX_LINEAR]; // hidden biases, padded
-    int s_wlt[PJ_MAX_NETS];              // [hpL][n_out]      last Linear, K-major        (forward)
-    int s_wlo[PJ_MAX_NETS];              // [n_out][hpL]      last Linear, out-major      (backward)
-    int s_bout[PJ_MAX_NETS];
-    long long b_wt[PJ_MAX_NETS][PJ_MAX_LINEAR];   // hidden->hidden Linear l: [in_p][out_p]  (forward B operand)
-    long long b_wo[PJ_MAX_NETS][PJ_MAX_LINEAR];   //                          [out_p][in_p]  (adjoint B operand)
-    long long b_wimg[PJ_MAX_NETS][PJ_MAX_LINEAR];   // tensor-core path: 3 bf16 split images of W_l, K-major SWIZZLE_128B (float offset)
-    long long b_woutimg[PJ_MAX_NETS];    // tensor-core path: 3 bf16 split images [16 x 64] of the output Linear (rows >= n_out zero)
-    int tc;                              // 1: K1 runs the hidden-layer and output GEMMs on wgmma (pinnjet_k1tc3.cuh)
-    int tc_bwd;                          // 1: K2 too (pinnjet_k2tc2.cuh); it reads K1-TC's records in place
-    int tp;                              // tensor-core tile: points per 128 GEMM rows (pinnjet_tc.cuh: TcGeo::TP)
-    int seed_T;                          // tile size of the seed / combined-weight layouts K1 writes ( = tp when tc_bwd, else T)
-    long long tc_rec_layer_floats, tc_rec_tile_floats;   // tensor-core record layout [tile][hidden layer][thread][C*UG]
-    long long ws_tcrec;                  // workspace offset (bytes) of those records
-    long long pack_floats;
-    // ---- small-gradient accumulators in shared memory (float offsets) ----
-    int g_w0[PJ_MAX_NETS], g_b[PJ_MAX_NETS][PJ_MAX_LINEAR], g_wl[PJ_MAX_NETS], g_bout[PJ_MAX_NETS], sgrad_floats;
-    int sgrad_copies;                    // one private copy per point-group block of warps (no atomics)
-    // ---- workspace (byte offsets) ----
-    int zj_off[PJ_MAX_NETS][PJ_MAX_LINEAR];       // float offset of hidden layer h (1..L) z-jets inside a tile block
-    long long zj_tile_floats;
-    long long ws_zj, ws_seed, ws_gpart, ws_loss, ws_bytes;
-    // ---- shared memory (byte offsets) ----
-    int k1_act, k1_ring, k1_small, k1_ycache, k1_slots, k1_prog, k1_misc, k1_bytes, k1_stage;
-    int k1_wbuf, k1_wslots, k1_progw;    // combined second-order channel: per-point weights, their interpreter state
-    long long ws_wts;                    // workspace: weights [tile][n_nets*wl][T] for K2
-    int k2_g0, k2_g1, k2_zb, k2_ring, k2_small, k2_ybar, k2_sgrad, k2_misc, k2_bytes;
 };
 
 struct K1Args {
@@ -114,7 +71,6 @@ struct K1Args {
     float* u_out;
     float* r_out;
     float* zj;                           // z-jet records (tensor-core layout when plan.tc)
-    float* zj_ffma;                      // plan.tc && !plan.tc_bwd: where the re-laid-out copy for the FFMA reverse kernel goes
     float* seeds;
     float* wts;
     float* loss_part;
@@ -144,17 +100,17 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
-// Programmatic dependent launch (K0 -> K1 -> finalize -> K2 -> K2b are launched with programmatic stream serialization, see
+// Programmatic dependent launch (K0 -> K1 -> K2 -> K2b are launched with programmatic stream serialization, see
 // launch_kernel below): a kernel lets its successor's CTAs become resident right away (they take the SMs as this grid's
 // CTAs retire), and the successor blocks in pdl_wait() -- until this grid has COMPLETED and its memory is visible -- before it
 // touches anything this grid writes.  Without the launch attribute both are no-ops.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// Loss finalisation inside the forward kernel (was a launch of its own): a program warp has stored its partial sum of
-// squared residuals; the warp that draws the last ticket adds ALL partials in the fixed order of the former
-// loss_finalize_kernel (lane-strided, then an xor-shuffle tree: run-to-run reproducible, identical numbers) to *sumsq_out and
-// re-arms the counter.  Called by whole warps; `lane0_stored` = lane 0 has written part[my index].
+// Loss finalisation inside the forward kernel: a program warp has stored its partial sum of squared residuals; the warp
+// that draws the last ticket adds ALL partials to *sumsq_out and re-arms the counter.  Fixed summation order, so the result
+// is run-to-run reproducible: lane l sums partials l, l + 32, l + 64, ... in that order, then the 32 lane sums are combined
+// by an xor-shuffle tree (offsets 16, 8, 4, 2, 1).  Called by whole warps after lane 0 has written part[my index].
 __device__ __forceinline__ void fold_loss_partials(const float* part, unsigned n_parts, float* sumsq_out, unsigned* ticket, int lane) {
     if (sumsq_out == nullptr) return;
     unsigned last = 0;

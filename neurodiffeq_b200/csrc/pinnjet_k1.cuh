@@ -104,7 +104,7 @@ __device__ __forceinline__ void finish_unit(float (&zq)[P][1 + N1 + N2], int act
 }
 
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL>
-__global__ void __launch_bounds__(NTC + (NTC == 128 ? 32 : 64), MINB) k1_forward_kernel(const __grid_constant__ K1Args A) {
+__global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(const __grid_constant__ K1Args A) {
     constexpr int C = 1 + N1 + N2;
     // service warps after the compute warps: 128-thread CTAs (weights always resident: the producer only issues the initial
     // loads) use ONE warp as producer-then-program warp; 256-thread CTAs have a producer warp and a program warp

@@ -25,10 +25,7 @@
 
 namespace pj {
 
-constexpr int K1T_NPW = 2;                                   // program warps
-constexpr int K1T_THREADS = TC_NT + 32 + 32 * K1T_NPW + 32;  // 640
-constexpr int K1T_EB = 32 * K1T_NPW;                         // points per program batch (a whole number of tiles)
-constexpr int K1T_RING = 4;                                  // tile buffers of the prefetch warp
+// K1T_THREADS (640), K1T_NPW (program warps), K1T_EB (points per program batch), K1T_RING: pinnjet_plan.h
 
 // JIT = true (csrc/pinnjet_jit.cu, neurodiffeq_b200/jit.py): the three programs of the problem are compiled into the kernel
 // as straight-line code (pj_jit_program_train / _eval / _w) instead of being interpreted.
@@ -78,7 +75,7 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
     for (int n = 0; n < sp.n_nets; ++n) n_hh += sp.net[n].n_linear - 2;
     unsigned char* woutimg = wimg + (size_t)n_hh * 3 * TC_WIMG;
     const bool train = A.mode == 1;
-    const int sT = pl.seed_T;                                        // tile size of the seed / weight layouts K2 reads
+    const int sT = pl.tp;                                            // tile size of the seed / weight layouts K2 reads
     const long long ws_points = (long long)pl.n_tiles * pl.T;
 
     pdl_launch_dependents();
@@ -388,36 +385,6 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
 template <int N1, int N2, int WL>
 __global__ void __launch_bounds__(K1T_THREADS, 1) k1tc3_forward_kernel(const __grid_constant__ K1Args A) {
     k1tc3_body<N1, N2, WL, false>(A);
-}
-
-// Bring-up / isolation helper (PINNJET_TC=1): copies the tensor-core records [tile][layer][thread][C*UG] into the layout
-// the FFMA reverse kernel reads ([K2 tile][net][hidden layer][unit][C*T + 4]).  One block per (tile, hidden layer).
-template <int C>
-__global__ void __launch_bounds__(TC_NT) tc_relayout_records_kernel(const __grid_constant__ K1Args A, const float* __restrict__ src,
-                                                                   float* __restrict__ dst) {
-    using G = TcGeo<C>;
-    const PjSpec& sp = A.spec;
-    const Plan& pl = A.plan;
-    int n_hidden = 0;
-    for (int n = 0; n < sp.n_nets; ++n) n_hidden += sp.net[n].n_linear - 1;
-    const long long tile = blockIdx.x / n_hidden;
-    int lidx = blockIdx.x % n_hidden, n = 0;
-    while (lidx >= sp.net[n].n_linear - 1) {
-        lidx -= sp.net[n].n_linear - 1;
-        ++n;
-    }
-    const int h = lidx + 1, T2 = pl.T, RS2 = pl.RS;
-    const TcThread<C> th(threadIdx.x);
-    const long long gp = tile * G::TP + th.p;
-    if (gp >= (long long)pl.n_tiles * T2) return;
-    float v[C][G::UG];
-    tc_load_record<C>(src + tile * pl.tc_rec_tile_floats + (size_t)(blockIdx.x % n_hidden) * pl.tc_rec_layer_floats +
-                          (size_t)threadIdx.x * G::REC, v);
-    float* out = dst + (gp / T2) * pl.zj_tile_floats + pl.zj_off[n][h] + (gp % T2);
-#pragma unroll
-    for (int k = 0; k < G::UG; ++k)
-#pragma unroll
-        for (int c = 0; c < C; ++c) out[(size_t)(th.ubase + k) * RS2 + c * T2] = v[c][k];
 }
 
 }  // namespace pj

@@ -41,7 +41,7 @@ __device__ __forceinline__ void wgrad_tile(f2 (&acc)[WJ][WK], const float* __res
 }
 
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL>
-__global__ void __launch_bounds__(NTC + 32, MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
+__global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
     constexpr int C = 1 + N1 + N2;
     constexpr int NT_COMPUTE = NTC, NT_TOTAL = NTC + 32, N_CWARPS = NTC / 32;
     extern __shared__ __align__(128) unsigned char smem[];

@@ -28,7 +28,6 @@
 
 namespace pj {
 
-constexpr int K2T_THREADS = TC_NT + 64;   // 576: compute warps, weight-load warp, record warp
 #ifndef PJ_WG_FIRST
 #define PJ_WG_FIRST 0                      // first split product of the weight-gradient GEMM (0: all six, 3: the three largest)
 #endif

@@ -22,21 +22,11 @@
 
 namespace pj {
 
-constexpr int TC_ROWS = 128;             // GEMM rows per tile
-constexpr int TC_H = 64;                 // hidden width
-constexpr int TC_AIMG = TC_ROWS * 128;   // bytes of one split image of a tile (128 rows x 64 bf16)
-constexpr int TC_WIMG = TC_H * 128;      // bytes of one split image of a hidden->hidden weight matrix
-constexpr int TC_WOUT = 16 * 128;        // bytes of one split image of an output layer (16 rows: outputs, zero padded)
-constexpr int TC_NCW = 16;               // compute warps
-constexpr int TC_NT = TC_NCW * 32;       // compute threads
-constexpr int TC_STAGE_STRIDE = 20;      // floats per staged accumulator row (16 + 4): row reads (16 B per lane) are
-                                         // conflict-free, fragment stores and owner-layout reads at most 2-way
-                                         // (tests/test_tc_layout.py)
-constexpr int TC_STAGE_BYTES = TC_NCW * 32 * TC_STAGE_STRIDE * 4;   // one private 32 x 16 block per compute warp
+// Tile, image and staging sizes, thread counts: pinnjet_plan.h (TC_*).
 
 template <int C>
 struct TcGeo {
-    static constexpr int CP = C <= 2 ? 2 : (C <= 4 ? 4 : 8);   // channels padded to a divisor of 32
+    static constexpr int CP = tc_channel_pad(C);               // channels padded to a divisor of 32
     static constexpr int TP = TC_ROWS / CP;                    // points per tile
     static constexpr int PW = 32 / CP;                         // points per 32-row warp block
     static constexpr int NUG = 32 / PW;                        // unit groups per 16-unit block: 2 / 4 / 8

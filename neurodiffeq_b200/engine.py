@@ -198,7 +198,7 @@ class FusedProblem:
         self.kernel_launches = 0
         self._graphs = {}
         self._jit, self._jit_ok, self.jit_reason = None, {}, "not requested"
-        # program-length limits of the kernels (pinnjet_api.cu: PROG_MAX, TC_PROG_RESERVE), checked here so that a residual the
+        # program-length limits of the kernels (pinnjet_plan.h: PROG_MAX, TC_PROG_RESERVE), checked here so that a residual the
         # kernels cannot hold is a fallback reason at construction rather than an error at the first batch
         longest = max(len(tp.prog_eval), len(tp.prog_train), len(tp.prog_train_ext))
         if longest > 1024:
