@@ -37,6 +37,7 @@ extern "C" {
 
 #define PJ_ABI_VERSION 2
 #define PJ_MAX_NETS 4
+#define PJ_MAX_OUT 32     /* output units per network (the tensor-core kernels take at most 4) */
 #define PJ_MAX_LINEAR 8   /* nn.Linear layers per network (hidden layers + 1) */
 #define PJ_MAX_COORDS 8
 #define PJ_MAX_DIRS 4     /* first-order jet directions */

@@ -13,7 +13,8 @@ User-supplied boundary callables (``x_min_val=lambda y: torch.sin(np.pi*y)`` ...
 Implemented: NoCondition :205-222, IVP :225-267, BundleIVP :270-345, DirichletBVP :398-435,
 BundleDirichletBVP :348-395, DirichletBVP2D :438-509, IBVP1D Dirichlet-Dirichlet :661-681,
 IBVP1D with Neumann data on one or both ends :670-701, DoubleEndedBVP1D :715-883, DirichletBVPSpherical :887-956,
-InfDirichletBVPSpherical :960-1019.  The Neumann flavours evaluate the network AT a boundary abscissa
+InfDirichletBVPSpherical :960-1019, DirichletBVPSphericalBasis :1023-1095, InfDirichletBVPSphericalBasis :1098-1166.
+The Neumann flavours evaluate the network AT a boundary abscissa
 (conditions.py:585-596, 823-834): traced as a second instance of the same network fed by a constant coordinate.
 """
 import warnings
@@ -41,6 +42,17 @@ def _traced_raw_output(g, net, n, o, coordinates):
         for i, c in enumerate(coordinates):
             out = out + g.theta(("skip", id(net), o, i)) * c
     return out
+
+
+def _register_net(net, coordinates):
+    """(graph, network index) of ``net`` fed by the traced coordinates ``coordinates``."""
+    g = coordinates[0].g
+    in_coord = []
+    for c in coordinates:
+        if not isinstance(c, _sym.Sym) or c.op != "coord":
+            raise NotImplementedError("fused enforce(): the network inputs must be the sampled coordinates")
+        in_coord.append(c.imm)
+    return g, g.register_net(net, in_coord)
 
 
 class BaseCondition:
@@ -103,13 +115,7 @@ class EnsembleCondition(BaseCondition):
     def enforce(self, net, *coordinates):
         if not _sym.is_symbolic(*coordinates):
             return self.parameterize(net(torch.cat(coordinates, dim=1)), *coordinates)
-        g = coordinates[0].g
-        in_coord = []
-        for c in coordinates:
-            if not isinstance(c, _sym.Sym) or c.op != "coord":
-                raise NotImplementedError("fused enforce(): the network inputs must be the sampled coordinates")
-            in_coord.append(c.imm)
-        n = g.register_net(net, in_coord)
+        g, n = _register_net(net, coordinates)
         return _sym.SymColumns([con.parameterize(_traced_raw_output(g, net, n, i, coordinates), *coordinates)
                                 for i, con in enumerate(self.conditions)])
 
@@ -366,3 +372,56 @@ class InfDirichletBVPSpherical(BaseCondition):
         dr = r - self.r_0
         decay, rise = _exp(-self.order * dr), dr.tanh()
         return self.f(theta, phi) * decay + self.g(theta, phi) * rise + decay * rise * output_tensor
+
+
+class _SphericalBasisCondition(BaseCondition):
+    """A condition on a network that takes only ``r`` and returns the K coefficients ``R_k(r)`` of a function basis
+    (``u = sum_k R_k(r) Y_k(theta, phi)``).  ``enforce(net, r)`` re-parameterises every output column; traced, the result
+    is a :class:`symbolic.SymColumns` with one column per network output, the boundary values applied per column."""
+
+    def enforce(self, net, r):
+        if not _sym.is_symbolic(r):
+            return self.parameterize(net(r), r)
+        from .tracing import NetDescription
+        g, n = _register_net(net, (r,))
+        n_out = NetDescription(net, (r.imm,)).n_out
+        return self.parameterize(_sym.SymColumns([_traced_raw_output(g, net, n, o, (r,)) for o in range(n_out)]), r)
+
+
+def _like(value, ref):
+    """A boundary-value tensor on the device / dtype of an eager network output (traced blocks take it as it is)."""
+    return value.to(ref) if isinstance(value, torch.Tensor) and isinstance(ref, torch.Tensor) else value
+
+
+class DirichletBVPSphericalBasis(_SphericalBasisCondition):
+    """R(r_0) = R_0 and, if given, R(r_1) = R_1 for the vector of basis coefficients R (reference conditions.py:1023-1095).
+    ``max_degree`` is deprecated and ignored."""
+
+    def __init__(self, r_0, R_0, r_1=None, R_1=None, max_degree=None):
+        super().__init__()
+        if (r_1 is None) ^ (R_1 is None):
+            raise ValueError(f'r_1 and R_1 must be both/neither set to None; got r_1={r_1}, R_1={R_1}')
+        self.r_0, self.r_1 = r_0, r_1
+        self.R_0, self.R_1 = R_0, R_1
+
+    def parameterize(self, output_tensor, r):
+        R_0, R_1 = _like(self.R_0, output_tensor), _like(self.R_1, output_tensor)
+        if self.r_1 is None:
+            return (1 - _exp(-r + self.r_0)) * output_tensor + R_0
+        rt = (r - self.r_0) / (self.r_1 - self.r_0)
+        return R_0 * (1 - rt) + R_1 * rt + (1. - _exp((1 - rt) * rt)) * output_tensor
+
+
+class InfDirichletBVPSphericalBasis(_SphericalBasisCondition):
+    """R(r_0) = R_0 and R(r -> inf) = R_inf with decay order ``order`` (reference conditions.py:1098-1166).
+    ``max_degree`` is deprecated and ignored."""
+
+    def __init__(self, r_0, R_0, R_inf, order=1, max_degree=None):
+        super().__init__()
+        self.r_0, self.R_0, self.R_inf, self.order = r_0, R_0, R_inf, order
+
+    def parameterize(self, output_tensor, r):
+        dr = r - self.r_0
+        decay = _exp(-self.order * dr)
+        R_0, R_inf = _like(self.R_0, output_tensor), _like(self.R_inf, output_tensor)
+        return R_0 * decay + R_inf * dr.tanh() + decay * dr.tanh() * output_tensor

@@ -175,8 +175,8 @@ __global__ void pack_kernel(const __grid_constant__ PackArgs A, const float* __r
             wlo[e] = (k2 < fin) ? W[o2 * fin + k2] : 0.0f;
         }
         float* bo = pack + pl.s_bout[n];
-        for (int o = tid; o < 4; o += nt) bo[o] = (o < fout) ? b[o] : 0.0f;
-        if (hpL == TC_H)   // rows = outputs (zero padded to 16), K = hidden unit
+        for (int o = tid; o < (fout + 3) / 4 * 4; o += nt) bo[o] = (o < fout) ? b[o] : 0.0f;   // region padded to 4
+        if (hpL == TC_H && fout <= 4)   // rows = outputs (zero padded to 16), K = hidden unit: nets the tensor cores can take
             pack_bf16x3_image(reinterpret_cast<unsigned char*>(pack + pl.b_woutimg[n]), W, 16, fout, fin, tid, nt);
     }
 }

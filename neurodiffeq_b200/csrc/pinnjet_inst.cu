@@ -76,11 +76,19 @@ static Variant<K2Args> k2_variant(const Plan& pl) {
         static const auto v = variant(k2tc2_backward_kernel<PJ_N1, PJ_N2, PJ_WL>, K2T_THREADS);
         return v;
     }
-    if (pl.ntc == 128) {
-        static const auto v = variant(k2_backward_kernel<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL>, ffma_k2_threads(128));
+    if (pl.n_out_max > K2_OUT_GROUP) {
+        if (pl.ntc == 128) {
+            static const auto v = variant(k2_backward_kernel<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, true>, ffma_k2_threads(128));
+            return v;
+        }
+        static const auto v = variant(k2_backward_kernel<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, true>, ffma_k2_threads(256));
         return v;
     }
-    static const auto v = variant(k2_backward_kernel<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL>, ffma_k2_threads(256));
+    if (pl.ntc == 128) {
+        static const auto v = variant(k2_backward_kernel<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, false>, ffma_k2_threads(128));
+        return v;
+    }
+    static const auto v = variant(k2_backward_kernel<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, false>, ffma_k2_threads(256));
     return v;
 }
 

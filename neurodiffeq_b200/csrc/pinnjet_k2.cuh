@@ -40,7 +40,8 @@ __device__ __forceinline__ void wgrad_tile(f2 (&acc)[WJ][WK], const float* __res
     }
 }
 
-template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL>
+// WIDE: some net has more than K2_OUT_GROUP outputs (a separate instance: the <= 4-output code stays as it is)
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, bool WIDE>
 __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
     constexpr int C = 1 + N1 + N2;
     constexpr int NT_COMPUTE = NTC, NT_TOTAL = NTC + 32, N_CWARPS = NTC / 32;
@@ -127,18 +128,22 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
             zphase ^= 1u;
             PJ_T_MARK(1)
 
-            // (1) last Linear: grads of W_out, b_out; adjoint of hidden-L a-jets; reverse activation -> G = z_bar_L
+            // (1) last Linear: grads of W_out, b_out; adjoint of hidden-L a-jets; reverse activation -> G = z_bar_L.
+            // WIDE instances (a net with more than K2_OUT_GROUP outputs): the adjoint sums over all outputs, the hidden-L
+            // a-jets replace the z-jets in Zb (each (unit, point) element belongs to one thread), then one pass per group
+            // of K2_OUT_GROUP outputs reduces W_out rows two at a time.
             {
                 const float* wlo = small + pl.s_wlo[n];
-                if (u0 < hpL) {
+                if constexpr (!WIDE) if (u0 < hpL) {
                     static_assert(Q == 4, "the gradient reductions below assume 4 units per thread");
-                    float gbq[Q], gwq[PJ_MAX_NETS][Q];   // per-thread partials: bias of hidden L, W_out (n_out <= 4)
+                    static_assert(K2_OUT_GROUP == PJ_MAX_NETS, "the first group's reduction below is written for 4 outputs");
+                    float gbq[Q], gwq[K2_OUT_GROUP][Q];   // per-thread partials: bias of hidden L, W_out rows of one group
 #pragma unroll
                     for (int q = 0; q < Q; ++q) {
                         const int u = u0 + q;
-                        float gw[PJ_MAX_NETS];
+                        float gw[K2_OUT_GROUP];
 #pragma unroll
-                        for (int o = 0; o < PJ_MAX_NETS; ++o) gw[o] = 0.0f;
+                        for (int o = 0; o < K2_OUT_GROUP; ++o) gw[o] = 0.0f;
                         float gb = 0.0f;
 #pragma unroll
                         for (int p = 0; p < P; ++p) {
@@ -150,7 +155,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                                 ab[c] = 0.0f;
                             }
 #pragma unroll
-                            for (int o = 0; o < PJ_MAX_NETS; ++o)
+                            for (int o = 0; o < K2_OUT_GROUP; ++o)
                                 if (o < n_out) {
                                     const float w = wlo[o * hpL + u];
 #pragma unroll
@@ -158,7 +163,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                                 }
                             act_backward<N1, N2, WL>(act_kind, z, ab, a, zb, wq[p]);
 #pragma unroll
-                            for (int o = 0; o < PJ_MAX_NETS; ++o)
+                            for (int o = 0; o < K2_OUT_GROUP; ++o)
                                 if (o < n_out) {
 #pragma unroll
                                     for (int c = 0; c < C; ++c) gw[o] = fmaf(ybar[(o * C + c) * T + pt], a[c], gw[o]);
@@ -169,10 +174,10 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                         }
                         gbq[q] = gb;
 #pragma unroll
-                        for (int o = 0; o < PJ_MAX_NETS; ++o) gwq[o][q] = gw[o];
+                        for (int o = 0; o < K2_OUT_GROUP; ++o) gwq[o][q] = gw[o];
                     }
+                    const int pl8 = jm.pg_lane, i4 = pl8 & 3;
                     {   // reduce over the point lanes: [bias(4) | W_out row 0 (4)], then W_out rows 1.. two at a time
-                        const int pl8 = jm.pg_lane, i4 = pl8 & 3;
                         const float v0[8] = {gbq[0], gbq[1], gbq[2], gbq[3], gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3]};
                         const float t0 = pg_reduce_scatter8(v0, pl8);
                         if (pl8 < 4) sg[pl.g_b[n][L - 1] + u0 + i4] += t0; else sg[pl.g_wl[n] + u0 + i4] += t0;
@@ -187,6 +192,76 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                             const float v2[4] = {gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
                             const float t2 = pg_reduce_scatter4(v2, pl8);
                             if (!(pl8 & 1)) sg[pl.g_wl[n] + 3 * hpL + u0 + (pl8 >> 1)] += t2;
+                        }
+                    }
+                }
+                if constexpr (WIDE) if (u0 < hpL) {
+                    float gbq[Q];
+#pragma unroll
+                    for (int q = 0; q < Q; ++q) {
+                        const int u = u0 + q;
+                        float gb = 0.0f;
+#pragma unroll
+                        for (int p = 0; p < P; ++p) {
+                            const int pt = p0 + p;
+                            float z[C], ab[C], a[C], zb[C];
+#pragma unroll
+                            for (int c = 0; c < C; ++c) {
+                                z[c] = Zb[u * RS + c * T + pt];
+                                ab[c] = 0.0f;
+                            }
+                            for (int o = 0; o < n_out; ++o) {
+                                const float w = wlo[o * hpL + u];
+#pragma unroll
+                                for (int c = 0; c < C; ++c) ab[c] = fmaf(w, ybar[(o * C + c) * T + pt], ab[c]);
+                            }
+                            act_backward<N1, N2, WL>(act_kind, z, ab, a, zb, wq[p]);
+                            gb += zb[0];
+#pragma unroll
+                            for (int c = 0; c < C; ++c) {
+                                G[u * RS + c * T + pt] = zb[c];
+                                Zb[u * RS + c * T + pt] = a[c];
+                            }
+                        }
+                        gbq[q] = gb;
+                    }
+                    const int pl8 = jm.pg_lane, i4 = pl8 & 3;
+                    const float tb = pg_reduce_scatter4(gbq, pl8);
+                    if (!(pl8 & 1)) sg[pl.g_b[n][L - 1] + u0 + (pl8 >> 1)] += tb;
+                    for (int o0 = 0; o0 < n_out; o0 += K2_OUT_GROUP) {
+                        float gwq[K2_OUT_GROUP][Q];
+#pragma unroll
+                        for (int q = 0; q < Q; ++q) {
+                            const int u = u0 + q;
+                            float gw[K2_OUT_GROUP];
+#pragma unroll
+                            for (int o = 0; o < K2_OUT_GROUP; ++o) gw[o] = 0.0f;
+#pragma unroll
+                            for (int p = 0; p < P; ++p) {
+                                const int pt = p0 + p;
+                                float a[C];
+#pragma unroll
+                                for (int c = 0; c < C; ++c) a[c] = Zb[u * RS + c * T + pt];
+#pragma unroll
+                                for (int o = 0; o < K2_OUT_GROUP; ++o)
+                                    if (o0 + o < n_out) {
+#pragma unroll
+                                        for (int c = 0; c < C; ++c) gw[o] = fmaf(ybar[((o0 + o) * C + c) * T + pt], a[c], gw[o]);
+                                    }
+                            }
+#pragma unroll
+                            for (int o = 0; o < K2_OUT_GROUP; ++o) gwq[o][q] = gw[o];
+                        }
+                        const int row = o0 + (pl8 >> 2);   // reduced value pl8: unit u0 + (pl8 & 3) of row o0 (+1 for pl8 >= 4)
+                        const float v1[8] = {gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3],
+                                             gwq[1][0], gwq[1][1], gwq[1][2], gwq[1][3]};
+                        const float t1 = pg_reduce_scatter8(v1, pl8);
+                        if (row < n_out) sg[pl.g_wl[n] + row * hpL + u0 + i4] += t1;
+                        if (o0 + 2 < n_out) {
+                            const float v2[8] = {gwq[2][0], gwq[2][1], gwq[2][2], gwq[2][3],
+                                                 gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
+                            const float t2 = pg_reduce_scatter8(v2, pl8);
+                            if (row + 2 < n_out) sg[pl.g_wl[n] + (row + 2) * hpL + u0 + i4] += t2;
                         }
                     }
                 }

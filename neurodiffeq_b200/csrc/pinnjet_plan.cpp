@@ -11,6 +11,13 @@ namespace pj {
 static int round_up(int v, int m) { return (v + m - 1) / m * m; }
 static long long round_up_ll(long long v, long long m) { return (v + m - 1) / m * m; }
 
+static int max_outputs(const PjSpec& sp) {   // widest output Linear of all nets
+    int m = 0;
+    for (int i = 0; i < sp.n_nets; ++i)
+        if (sp.net[i].width[sp.net[i].n_linear] > m) m = sp.net[i].width[sp.net[i].n_linear];
+    return m;
+}
+
 static int hidden_linears(const PjSpec& sp) {   // hidden->hidden Linears of all nets
     int n = 0;
     for (int i = 0; i < sp.n_nets; ++i) n += sp.net[i].n_linear - 2;
@@ -45,7 +52,8 @@ int k2_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, SmemImage* regions) 
     img.place(pl.k2_zb, "zb", jet_bytes);
     img.place(pl.k2_ring, "ring", n_stage * CHUNK_FLOATS * 4);
     img.place(pl.k2_small, "small", round_up(pl.small_floats * 4, 128));
-    img.place(pl.k2_ybar, "ybar", round_up(PJ_MAX_NETS * pl.C * pl.T * 4, 128));
+    const int ybar_rows = pl.n_out_max > K2_OUT_GROUP ? pl.n_out_max : K2_OUT_GROUP;
+    img.place(pl.k2_ybar, "ybar", round_up(ybar_rows * pl.C * pl.T * 4, 128));
     img.place(pl.k2_sgrad, "sgrad", round_up(pl.sgrad_floats * pl.sgrad_copies * 4, 128));
     img.place(pl.k2_misc, "misc", 256);
     if (regions) *regions = img;
@@ -137,7 +145,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     if (sp.n_coords < 1 || sp.n_coords > PJ_MAX_COORDS) return fail(-1, "n_coords=%d out of range", sp.n_coords);
     if (N < 1) return fail(-1, "n_points must be positive");
     if (prog_len > PROG_MAX) return fail(-2, "residual program too long (%d > %d instructions)", prog_len, PROG_MAX);
-    if (sp.n_slots < 1 || sp.n_slots > 64) return fail(-2, "n_slots=%d out of range (1..64)", sp.n_slots);
+    if (sp.n_slots < 1 || sp.n_slots > SLOTS_MAX) return fail(-2, "n_slots=%d out of range (1..%d)", sp.n_slots, SLOTS_MAX);
     if (sp.wl < 0 || sp.wl > sp.n1 || (sp.wl > 0 && sp.n2 != 1)) return fail(-1, "inconsistent wl=%d (n1=%d, n2=%d)", sp.wl, sp.n1, sp.n2);
     const int C = 1 + sp.n1 + sp.n2;
     pl.C = C;
@@ -149,7 +157,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
         if (net.n_linear < 2 || net.n_linear > PJ_MAX_LINEAR) return fail(-1, "net %d: n_linear=%d out of range", n, net.n_linear);
         if (net.n_in < 1 || net.n_in > PJ_MAX_COORDS || net.width[0] != net.n_in) return fail(-1, "net %d: bad n_in", n);
         const int n_out = net.width[net.n_linear];
-        if (n_out < 1 || n_out > PJ_MAX_NETS) return fail(-2, "net %d: %d output units (max %d)", n, n_out, PJ_MAX_NETS);
+        if (n_out < 1 || n_out > PJ_MAX_OUT) return fail(-2, "net %d: %d output units (max %d)", n, n_out, PJ_MAX_OUT);
         if (net.act != PJ_ACT_TANH && net.act != PJ_ACT_SIN) return fail(-2, "net %d: unknown activation", n);
         if (net.yrow0 != yrows) return fail(-1, "net %d: yrow0 must be %d", n, yrows);
         yrows += n_out * C;
@@ -164,8 +172,8 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
             if (pl.hp[n][h] > hmax) hmax = pl.hp[n][h];
         }
     }
+    pl.n_out_max = max_outputs(sp);
     if (yrows != sp.n_yrows) return fail(-1, "n_yrows=%d but the nets need %d", sp.n_yrows, yrows);
-    if (yrows > 32) return fail(-2, "jet table has %d rows (max 32)", yrows);
     if (hmax > 64) hmax = 128; else if (hmax > 32) hmax = 64;
     pl.hmax = hmax;
     pl.ntc = ntc_req;
@@ -191,7 +199,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
         for (int l = 0; l < L; ++l) { pl.s_b[n][l] = off; off += pl.hp[n][l + 1]; }
         pl.s_wlt[n] = off; off += round_up(pl.hp[n][L] * n_out, 4);
         pl.s_wlo[n] = off; off += round_up(pl.hp[n][L] * n_out, 4);
-        pl.s_bout[n] = off; off += 4;
+        pl.s_bout[n] = off; off += round_up(n_out, 4);
     }
     pl.small_floats = off;
     long long big = off;
@@ -218,16 +226,17 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
         pl.g_w0[n] = off; off += pl.hp[n][1] * net.n_in;
         for (int l = 0; l < L; ++l) { pl.g_b[n][l] = off; off += pl.hp[n][l + 1]; }
         pl.g_wl[n] = off; off += n_out * pl.hp[n][L];
-        pl.g_bout[n] = off; off += 4;
+        pl.g_bout[n] = off; off += round_up(n_out, 4);
     }
     pl.sgrad_floats = round_up(off, 4);
     pl.sgrad_copies = (pl.T / pl.P) / 8;
 
     // ---- kernel selection ----
-    // Tensor-core kernels (pinnjet_tc.cuh): every hidden layer exactly 64 wide (after padding), at most 8 jet channels, the
-    // weight images of both kernels resident in shared memory.  The decision may not depend on the program length (only
+    // Tensor-core kernels (pinnjet_tc.cuh): every hidden layer exactly 64 wide (after padding), at most 8 jet channels, at
+    // most 4 outputs per net (one 16-byte row of the output Linear), the weight images of both kernels resident in shared
+    // memory.  The decision may not depend on the program length (only
     // pj_forward* know it): the programs get a fixed reserve.
-    bool tc = dev.tc_level > 0 && C <= 8 && hmax == TC_H;
+    bool tc = dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4;
     for (int n = 0; tc && n < sp.n_nets; ++n)
         for (int h = 1; h < sp.net[n].n_linear; ++h) tc = tc && pl.hp[n][h] == TC_H;
     if (tc) {   // both kernels tile like the forward kernel; seeds / weights / records are shared as is

@@ -17,6 +17,8 @@ constexpr int ROW_PAD = 4;               // jet rows are C*T + 4 floats: conflic
 // Thread tile: P points x Q units.  K2 and narrow-network K1 CTAs use Q = FFMA_Q; K1 of 128-wide networks FFMA_Q_WIDE.
 constexpr int ffma_tile_points(int C) { return C <= 2 ? 4 : 2; }
 constexpr int FFMA_Q = 4, FFMA_Q_WIDE = 8;
+// K2 reduces the output-Linear gradient in groups of this many outputs (pinnjet_k2.cuh)
+constexpr int K2_OUT_GROUP = 4;
 // block = compute threads + service warps.  K1: 128-thread CTAs share one producer / program warp, 256-thread CTAs have
 // one of each; K2: one producer warp.
 constexpr int ffma_k1_threads(int ntc) { return ntc + (ntc == 128 ? 32 : 64); }
@@ -43,7 +45,8 @@ constexpr int K2T_THREADS = TC_NT + 64;                      // 576: compute war
 constexpr int TC_PROG_RESERVE = 8192;    // shared-memory bytes the tensor-core plan sets aside for the programs
 
 // ---- residual programs ----
-constexpr int PROG_MAX = 1024;           // instructions
+constexpr int PROG_MAX = 2048;           // instructions
+constexpr int SLOTS_MAX = 128;           // value-file entries per point
 
 // ---- workspace: the loss-partial block at its start ----
 constexpr int LOSS_PART_BYTES = 4096;
@@ -72,6 +75,7 @@ struct Plan {
     long long b_wo[PJ_MAX_NETS][PJ_MAX_LINEAR];   //                          [out_p][in_p]  (adjoint B operand)
     long long b_wimg[PJ_MAX_NETS][PJ_MAX_LINEAR];   // tensor-core path: 3 bf16 split images of W_l, K-major SWIZZLE_128B (float offset)
     long long b_woutimg[PJ_MAX_NETS];    // tensor-core path: 3 bf16 split images [16 x 64] of the output Linear (rows >= n_out zero)
+    int n_out_max;                       // widest output Linear of all nets (K2 instances with > K2_OUT_GROUP differ)
     int tc;                              // 1: K1 and K2 run the hidden-layer GEMMs on wgmma (pinnjet_k1tc3.cuh, pinnjet_k2tc2.cuh)
     int tp;                              // tensor-core tile: points per 128 GEMM rows (pinnjet_tc.cuh: TcGeo::TP)
     int n_loss_parts;                    // loss partials K1 writes: one per CTA (FFMA), one per program warp (K1-TC)

@@ -201,8 +201,8 @@ class FusedProblem:
         # program-length limits of the kernels (pinnjet_plan.h: PROG_MAX, TC_PROG_RESERVE), checked here so that a residual the
         # kernels cannot hold is a fallback reason at construction rather than an error at the first batch
         longest = max(len(tp.prog_eval), len(tp.prog_train), len(tp.prog_train_ext))
-        if longest > 1024:
-            raise NotImplementedError(f"residual program of {longest} instructions (the kernels hold 1024)")
+        if longest > 2048:
+            raise NotImplementedError(f"residual program of {longest} instructions (the kernels hold 2048)")
         if (longest + (len(tp.prog_w) if tp.wl else 0)) * 16 > 8192 and self.plan_info(1024).get("tc"):
             raise NotImplementedError(f"residual program of {longest} instructions is too long for the tensor-core forward kernel "
                                       f"(PINNJET_TC=0 runs this problem on the FFMA kernels)")

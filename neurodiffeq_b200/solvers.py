@@ -30,6 +30,7 @@ from .engine import FusedProblem
 from .eager import build_problem
 from ._compat import renamed_arguments
 from .losses import _losses, h1_rows, h1_semi_rows
+from .function_basis import RealSphericalHarmonics
 from .generators import Generator1D, Generator2D, GeneratorSpherical, SamplerGenerator
 from .networks import FCNN
 from .parallel import shard_bounds
@@ -675,6 +676,11 @@ class BaseSolver:
         return BaseSolution
 
     def get_solution(self, copy=True, best=True):
+        return self._solution(copy, best, lambda nets, conditions: self._solution_class()(
+            nets, conditions, self.n_coords, self._coords_for_condition, enforce=self.compute_func_val, device=self.device))
+
+    def _solution(self, copy, best, make):
+        """``make(nets, conditions)`` on the best or live networks, copied unless ``copy=False``."""
         nets = self.best_nets if best else self.nets
         if nets is None:
             raise RuntimeError("The nets cannot be None, check if you disabled validation "
@@ -686,8 +692,7 @@ class BaseSolver:
             conditions = deepcopy(conditions)
         elif best:
             warnings.warn("copy=False with best=True returns a copy of the best networks", RuntimeWarning)
-        return self._solution_class()(nets, conditions, self.n_coords, self._coords_for_condition,
-                                      enforce=self.compute_func_val, device=self.device)
+        return make(nets, conditions)
 
     def get_residuals(self, *coords, to_numpy=False, best=True, no_reshape=False):
         coords = [c if isinstance(c, torch.Tensor) else torch.as_tensor(np.asarray(c)) for c in coords]
@@ -746,6 +751,32 @@ class Solution2D(BaseSolution):
 
 class SolutionSpherical(BaseSolution):
     pass
+
+
+class SolutionSphericalHarmonics(SolutionSpherical):
+    """Solution ``u = sum_k R_k(r) Y_k(theta, phi)`` of networks that take only ``r`` and return the coefficients R_k of the
+    basis ``harmonics_fn`` (reference solvers.py:962-1012).  The sum is part of the traced function, so the forward
+    kernel evaluates it.  ``max_degree`` is deprecated: it selects ``RealSphericalHarmonics(max_degree)`` unless
+    ``harmonics_fn`` is given."""
+
+    def __init__(self, nets, conditions, max_degree=None, harmonics_fn=None, device=None):
+        super().__init__(nets, conditions, 3, enforce=self._compute_u, device=device)
+        if harmonics_fn is None and max_degree is None:
+            raise ValueError("harmonics_fn should be specified")
+        if max_degree is not None:
+            warnings.warn("`max_degree` is DEPRECATED; pass `harmonics_fn` instead, which takes precedence", FutureWarning)
+            self.harmonics_fn = RealSphericalHarmonics(max_degree=max_degree)
+        if harmonics_fn is not None:
+            self.harmonics_fn = harmonics_fn
+
+    def _compute_u(self, net, condition, rs, thetas, phis):
+        return torch.sum(condition.enforce(net, rs) * self.harmonics_fn(thetas, phis), dim=1)
+
+    def __call__(self, *coords, to_numpy=False, no_reshape=False):
+        us = super().__call__(*coords, to_numpy=to_numpy, no_reshape=no_reshape)
+        if no_reshape:   # the sum over the basis has shape (N,), as in the reference
+            us = [u.reshape(-1) for u in us] if isinstance(us, list) else us.reshape(-1)
+        return us
 
 
 class BundleSolution1D(BaseSolution):
@@ -854,6 +885,14 @@ class SolverSpherical(BaseSolver):
 
     def _solution_class(self):
         return SolutionSpherical
+
+    def get_solution(self, copy=True, best=True, harmonics_fn=None):
+        """A callable solution; with ``harmonics_fn`` the networks' outputs are the coefficients of that basis
+        (:class:`SolutionSphericalHarmonics`, reference solvers.py:933-957)."""
+        if harmonics_fn is None:
+            return super().get_solution(copy=copy, best=best)
+        return self._solution(copy, best, lambda nets, conditions: SolutionSphericalHarmonics(
+            nets, conditions, harmonics_fn=harmonics_fn, device=self.device))
 
     def _get_internal_variables(self):
         d = super()._get_internal_variables()

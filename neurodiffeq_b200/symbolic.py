@@ -309,30 +309,30 @@ class Sym:
         raise TypeError("the truth value of a traced (fused) expression is undefined; data-dependent Python control "
                         "flow cannot be fused into the residual kernel")
 
-    # -- arithmetic
+    # -- arithmetic (an (N, k) operand -- a traced block or k per-column constants -- makes the result a block)
     def __add__(self, o):
-        return self.g.add(self, o)
+        return _columns_binary("add", self, o) if _is_block(o) else self.g.add(self, o)
 
     def __radd__(self, o):
-        return self.g.add(o, self)
+        return _columns_binary("add", o, self) if _is_block(o) else self.g.add(o, self)
 
     def __sub__(self, o):
-        return self.g.sub(self, o)
+        return _columns_binary("sub", self, o) if _is_block(o) else self.g.sub(self, o)
 
     def __rsub__(self, o):
-        return self.g.sub(o, self)
+        return _columns_binary("sub", o, self) if _is_block(o) else self.g.sub(o, self)
 
     def __mul__(self, o):
-        return self.g.mul(self, o)
+        return _columns_binary("mul", self, o) if _is_block(o) else self.g.mul(self, o)
 
     def __rmul__(self, o):
-        return self.g.mul(o, self)
+        return _columns_binary("mul", o, self) if _is_block(o) else self.g.mul(o, self)
 
     def __truediv__(self, o):
-        return self.g.div(self, o)
+        return _columns_binary("div", self, o) if _is_block(o) else self.g.div(self, o)
 
     def __rtruediv__(self, o):
-        return self.g.div(o, self)
+        return _columns_binary("div", o, self) if _is_block(o) else self.g.div(o, self)
 
     def __neg__(self):
         return self.g.neg(self)
@@ -422,8 +422,12 @@ class Sym:
 
 class SymColumns:
     """An (N, k) block of traced columns -- what ``EnsembleCondition.enforce`` returns for a k-output network
-    (reference conditions.py:197-202 concatenates the re-parameterised columns).  Supports what user code does with such
-    a tensor: ``u[:, i]``, ``u[:, i:i+1]`` (a column = a :class:`Sym`), ``u[:, i:j]`` (a narrower block), ``u.shape``."""
+    (reference conditions.py:197-202 concatenates the re-parameterised columns) and what the function-basis code builds
+    (reference function_basis.py).  Supports what user code does with such a tensor: ``u[:, i]``, ``u[:, i:i+1]`` (a
+    column = a :class:`Sym`), ``u[:, i:j]`` (a narrower block), ``u.shape``; element-wise ``+ - * / **`` with numbers,
+    (N, 1) columns, blocks of the same width and 1-D or (1, k) tensors / arrays (one constant per column); column-wise
+    unary functions; ``torch.cat(..., dim=1)``; ``x.sum(dim=1)`` (a column); ``x.split(1, dim=1)``."""
+    __array_priority__ = 1000
 
     def __init__(self, cols):
         self.cols = tuple(cols)
@@ -466,6 +470,68 @@ class SymColumns:
     def __repr__(self):
         return f"SymColumns({len(self.cols)})"
 
+    def __hash__(self):
+        return id(self)
+
+    def __bool__(self):
+        raise TypeError("the truth value of a traced (fused) expression is undefined")
+
+    def __add__(self, o):
+        return _columns_binary("add", self, o)
+
+    def __radd__(self, o):
+        return _columns_binary("add", o, self)
+
+    def __sub__(self, o):
+        return _columns_binary("sub", self, o)
+
+    def __rsub__(self, o):
+        return _columns_binary("sub", o, self)
+
+    def __mul__(self, o):
+        return _columns_binary("mul", self, o)
+
+    def __rmul__(self, o):
+        return _columns_binary("mul", o, self)
+
+    def __truediv__(self, o):
+        return _columns_binary("div", self, o)
+
+    def __rtruediv__(self, o):
+        return _columns_binary("div", o, self)
+
+    def __pow__(self, p):
+        return _columns_binary("pow", self, p)
+
+    def __neg__(self):
+        return SymColumns([-c for c in self.cols])
+
+    def __pos__(self):
+        return self
+
+    def __abs__(self):
+        return _columns_unary("abs", (self,), {})
+
+    def sum(self, dim=None, keepdim=False):
+        return _columns_sum(self, dim)
+
+    def split(self, split_size, dim=0):
+        return _columns_split(self, split_size, dim)
+
+    def __getattr__(self, name):   # tensor methods that are column-wise unary functions: x.sin(), x.exp(), ...
+        if name in _COLUMNWISE_METHODS:
+            return lambda *a, **k: _columns_unary(name, (self,) + a, k)
+        raise AttributeError(name)
+
+    def __array_ufunc__(self, ufunc, method, *inputs, **kwargs):
+        if method != "__call__":
+            return NotImplemented
+        return _dispatch_function(ufunc.__name__, inputs, kwargs)
+
+    @classmethod
+    def __torch_function__(cls, func, types, args=(), kwargs=None):
+        return _dispatch_function(getattr(func, "__name__", str(func)), args, kwargs or {})
+
 
 class _SymShape(tuple):
     """Shape of a traced (N,1) column: compares equal to any other traced shape; index 1 is 1."""
@@ -489,7 +555,7 @@ _NAME_ALIASES = {"multiply": "mul", "true_divide": "div", "divide": "div", "subt
 
 def _first_graph(args):
     for a in args:
-        if isinstance(a, Sym):
+        if isinstance(a, (Sym, SymColumns)):
             return a.g
         if isinstance(a, (list, tuple)):
             g = _first_graph(a)
@@ -498,10 +564,137 @@ def _first_graph(args):
     return None
 
 
+_COLUMNWISE_METHODS = set(_UNARY) | {"square", "reciprocal", "rsqrt", "exp2", "sigmoid", "pow", "arctan", "absolute"}
+_DUNDER = {"__add__": ("add", False), "__radd__": ("add", True), "__sub__": ("sub", False), "__rsub__": ("sub", True),
+           "__mul__": ("mul", False), "__rmul__": ("mul", True), "__truediv__": ("div", False),
+           "__rtruediv__": ("div", True), "__div__": ("div", False), "__rdiv__": ("div", True), "__pow__": ("pow", False)}
+
+
+def _is_block(x):
+    """An (N, k) operand: a traced block, or a tensor / array of k > 1 per-column constants."""
+    return isinstance(x, SymColumns) or (isinstance(x, (torch.Tensor, np.ndarray)) and _numel(x) > 1)
+
+
+def _numel(x):
+    return x.numel() if isinstance(x, torch.Tensor) else x.size
+
+
+def _column_values(x, width):
+    """``x`` as a list of ``width`` per-column operands (numbers, Syms)."""
+    if isinstance(x, SymColumns):
+        if len(x.cols) == width:
+            return list(x.cols)
+        if len(x.cols) == 1:
+            return list(x.cols) * width
+        raise ValueError(f"traced blocks of widths {len(x.cols)} and {width} do not broadcast")
+    if isinstance(x, (torch.Tensor, np.ndarray)):
+        a = x.detach().cpu().double().numpy() if isinstance(x, torch.Tensor) else np.asarray(x, dtype=np.float64)
+        if a.size == 1:
+            return [float(a.reshape(-1)[0])] * width
+        if a.ndim == 1 or (a.ndim == 2 and a.shape[0] == 1):
+            a = a.reshape(-1)
+            if a.size == width:
+                return [float(v) for v in a]
+        raise NotImplementedError(f"a constant of shape {tuple(a.shape)} with a traced (N, {width}) block: only 1-D or "
+                                  f"(1, {width}) per-column constants are supported")
+    return [x] * width
+
+
+def _block_width(args):
+    widths = set()
+    for a in args:
+        if isinstance(a, SymColumns):
+            widths.add(len(a.cols))
+        elif isinstance(a, (torch.Tensor, np.ndarray)) and _numel(a) > 1:
+            widths.add(_numel(a))
+    widths.discard(1)
+    if len(widths) > 1:
+        raise ValueError(f"operands of widths {sorted(widths)} do not broadcast")
+    return widths.pop() if widths else 1
+
+
+def _columns_binary(name, a, b):
+    width = _block_width((a, b))
+    if not any(isinstance(x, (Sym, SymColumns)) for x in (a, b)):
+        raise TypeError("no traced operand")
+    g = _first_graph((a, b))
+    out = []
+    for x, y in zip(_column_values(a, width), _column_values(b, width)):
+        out.append(g.pow(x, y) if name == "pow" else getattr(g, name)(x, y))
+    return SymColumns(out)
+
+
+def _columns_unary(name, args, kwargs):
+    x = args[0]
+    return SymColumns([_dispatch_function(name, (c,) + tuple(args[1:]), kwargs) for c in x.cols])
+
+
+def _columns_sum(x, dim):
+    if dim not in (1, -1):
+        raise NotImplementedError("a traced (N, k) block can only be summed over its columns: sum(dim=1)")
+    out = x.cols[0]
+    for c in x.cols[1:]:
+        out = out + c
+    return out
+
+
+def _columns_split(x, split_size, dim):
+    if dim not in (1, -1):
+        raise NotImplementedError("a traced (N, k) block can only be split into columns: split(size, dim=1)")
+    if not isinstance(split_size, int) or split_size < 1:
+        raise NotImplementedError("split of a traced block: an integer chunk size only")
+    chunks = [x.cols[i:i + split_size] for i in range(0, len(x.cols), split_size)]
+    return tuple(c[0] if len(c) == 1 else SymColumns(c) for c in chunks)
+
+
+def _concat_columns(args, kwargs):
+    seq = args[0]
+    dim = kwargs.get("dim", kwargs.get("axis", args[1] if len(args) > 1 else 0))
+    if dim not in (1, -1):
+        raise NotImplementedError("torch.cat of traced columns: only along dim=1 (a block of columns); the network "
+                                  "inputs are concatenated by `condition.enforce(net, *coords)`")
+    cols = []
+    for x in seq:
+        if isinstance(x, SymColumns):
+            cols += list(x.cols)
+        elif isinstance(x, Sym):
+            cols.append(x)
+        else:
+            raise NotImplementedError(f"torch.cat of a traced column with {type(x).__name__}")
+    return SymColumns(cols)
+
+
 def _dispatch_function(name, args, kwargs):
-    """torch.<name>(...) / numpy.<name>(...) with at least one Sym argument."""
+    """torch.<name>(...) / numpy.<name>(...) with at least one Sym / SymColumns argument."""
     g = _first_graph(args)
     name = _NAME_ALIASES.get(name, name)
+    if name in _DUNDER:
+        op, swap = _DUNDER[name]
+        a, b = (args[1], args[0]) if swap else (args[0], args[1])
+        if _is_block(a) or _is_block(b):
+            return _columns_binary(op, a, b)
+        return g.pow(a, b) if op == "pow" else getattr(g, op)(a, b)
+    if name in ("cat", "concatenate", "concat"):
+        return _concat_columns(args, kwargs)
+    if name == "sum" and isinstance(args[0], SymColumns):
+        return _columns_sum(args[0], kwargs.get("dim", args[1] if len(args) > 1 else None))
+    if name == "split" and isinstance(args[0], SymColumns):
+        return _columns_split(args[0], args[1] if len(args) > 1 else kwargs.get("split_size_or_sections"),
+                              kwargs.get("dim", args[2] if len(args) > 2 else 0))
+    if name in ("add", "sub", "mul", "div", "pow", "atan2") and (_is_block(args[0]) or _is_block(args[1])):
+        if name in ("add", "sub") and kwargs.get("alpha", 1) != 1:
+            raise NotImplementedError("alpha= in traced add/sub")
+        if name == "atan2":
+            width = _block_width(args[:2])
+            return SymColumns([_dispatch_function("atan2", (y, x), {}) for y, x in
+                               zip(_column_values(args[0], width), _column_values(args[1], width))])
+        return _columns_binary(name, args[0], args[1])
+    if isinstance(args[0], SymColumns):
+        if name in _COLUMNWISE_METHODS:
+            return _columns_unary(name, args, kwargs)
+        if name in ("clone", "detach", "contiguous"):
+            return args[0]
+        raise NotImplementedError(f"`{name}` is not supported on a traced (N, k) block")
     if name in _UNARY:
         return g.unary(name, args[0])
     if name in ("add", "sub", "mul", "div"):
@@ -532,9 +725,8 @@ def _dispatch_function(name, args, kwargs):
         y, x = g.lift(args[0]), g.lift(args[1])
         r = g.unary("sqrt", g.add(g.mul(x, x), g.mul(y, y)))
         return g.mul(2.0, g.unary("atan", g.div(y, g.add(r, x))))
-    if name == "cat" or name == "concatenate" or name == "stack":
-        raise NotImplementedError("torch.cat of traced columns: only `condition.enforce(net, *coords)` may "
-                                  "concatenate coordinates (that is where the network input is recorded)")
+    if name == "stack":
+        raise NotImplementedError("torch.stack of traced columns")
     raise NotImplementedError(f"`{name}` is not supported inside a fused residual / condition expression")
 
 

@@ -270,6 +270,82 @@ def _biharmonic(nd):
                     make_conditions, diff_eqs, 1, 512, _fcnn_flops((2, 16, 16, 1), 15), None)
 
 
+# ----------------------------------------------------------------------------------------------------------------------
+# S1..S3  networks with more than 4 outputs: spherical-harmonic expansions u = sum_k R_k(r) Y_k(theta, phi) of a network
+# that sees only r (reference function_basis.py, conditions.py:1023-1166), and a 6-output ODE system
+# ----------------------------------------------------------------------------------------------------------------------
+def _gaussian_charge():
+    r0, r1 = 0.1, 3.0
+    k_q = 1.0 / (4 * math.pi)
+    return r0, r1, k_q / r0 * math.erf(r0 / math.sqrt(2)), k_q / r1 * math.erf(r1 / math.sqrt(2)), (2 * math.pi) ** 1.5
+
+
+def _s1(nd):
+    """The reference's Gaussian-charge problem on RealSphericalHarmonics(2): K = 9 coefficients, DirichletBVPSphericalBasis
+    and HarmonicsLaplacian (reference tests/test_pde_spherical.py:147-173)."""
+    r0, r1, v0, v1, norm = _gaussian_charge()
+    K = 9
+    laplacian = nd.HarmonicsLaplacian(max_degree=2)
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=K, hidden_units=(32, 32))]
+
+    def make_conditions():
+        R_0 = torch.tensor([v0 * 2] + [0.0] * (K - 1), dtype=torch.float64)
+        R_1 = torch.tensor([v1 * 2] + [0.0] * (K - 1), dtype=torch.float64)
+        return [nd.DirichletBVPSphericalBasis(r_0=r0, R_0=R_0, r_1=r1, R_1=R_1, max_degree=2)]
+
+    def diff_eqs(R, r, th, ph):
+        return [laplacian(R, r, th, ph) + torch.exp(-r ** 2 / 2) / norm]
+
+    return Workload("s1_harmonics_poisson", "SolverSpherical", ("r", "theta", "phi"),
+                    ((r0, r1), (0.07, math.pi - 0.07), (0.0, 2 * math.pi)), [((1, 32, 32, K), "tanh")], make_nets,
+                    make_conditions, diff_eqs, 1, 32768, _fcnn_flops((1, 32, 32, K), 3), None)
+
+
+def _s2(nd):
+    """Degree 4 (K = 25) with InfDirichletBVPSphericalBasis; the Laplacian written out in the reference's own style:
+    torch.cat of per-column derivatives, a coefficient tensor, torch.sum over the basis."""
+    r0, _, v0, _, norm = _gaussian_charge()
+    K = 25
+    harmonics = nd.RealSphericalHarmonics(max_degree=4)
+    coefficients = torch.tensor([-l * (l + 1) * 1.0 for l in range(5) for _ in range(2 * l + 1)])
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=K, hidden_units=(32, 32))]
+
+    def make_conditions():
+        return [nd.InfDirichletBVPSphericalBasis(r_0=r0, R_0=torch.tensor([v0 * 2] + [0.0] * (K - 1), dtype=torch.float64),
+                                                 R_inf=torch.zeros(K, dtype=torch.float64), order=1)]
+
+    def diff_eqs(R, r, th, ph):
+        radial = torch.cat([nd.diff(R[:, j:j + 1] * r, r, order=2) for j in range(R.shape[1])], dim=1) / r
+        angular = coefficients * R / r ** 2
+        return [torch.sum((radial + angular) * harmonics(th, ph), dim=1, keepdim=True) + torch.exp(-r ** 2 / 2) / norm]
+
+    return Workload("s2_harmonics_inf", "SolverSpherical", ("r", "theta", "phi"),
+                    ((r0, 3.0), (0.07, math.pi - 0.07), (0.0, 2 * math.pi)), [((1, 32, 32, K), "tanh")], make_nets,
+                    make_conditions, diff_eqs, 1, 32768, _fcnn_flops((1, 32, 32, K), 3), None)
+
+
+def _s3(nd):
+    """Solver1D, one 6-output network under an EnsembleCondition of 6 IVPs: the linear cycle u_i' = u_{i+1} - a_i u_i."""
+    K = 6
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=K, hidden_units=(32, 32))]
+
+    def make_conditions():
+        return [nd.EnsembleCondition(*[nd.IVP(t_0=0.0, u_0=1.0 - 0.2 * i) for i in range(K)])]
+
+    def diff_eqs(u, t):
+        cols = [u[:, i:i + 1] for i in range(K)]
+        return [nd.diff(cols[i], t) - cols[(i + 1) % K] + 0.5 * (i + 1) * cols[i] for i in range(K)]
+
+    return Workload("s3_ensemble_cycle", "Solver1D", ("t",), ((0.0, 2.0),), [((1, 32, 32, K), "tanh")], make_nets,
+                    make_conditions, diff_eqs, K, 4096, _fcnn_flops((1, 32, 32, K), 2), None)
+
+
 _EXTRA = {
     "x1": lambda nd: _heat(nd, "x1_heat_dirichlet_neumann", "right"),
     "x2": lambda nd: _heat(nd, "x2_heat_neumann_dirichlet", "left"),
@@ -289,6 +365,16 @@ _BUILDERS.update(_EXTRA)
 _FALLBACK = {"y1": _third_order, "y2": _softplus_net, "y3": _biharmonic}
 FALLBACK_NAMES = tuple(_FALLBACK)
 _BUILDERS.update(_FALLBACK)
+# networks with more than 4 outputs; kept out of the tuples above, which parametrise the existing tests
+_BASIS = {"s1": _s1, "s2": _s2, "s3": _s3}
+BASIS_NAMES = tuple(_BASIS)
+_BUILDERS.update(_BASIS)
+# workloads whose conditions see only the first coordinate (a network of r alone, as SolverSpherical passes it)
+_RADIAL = ("s1", "s2")
+
+
+def coords_for_condition(key):
+    return (lambda k, cond, coords: tuple(coords[:1])) if key in _RADIAL else None
 
 
 def build(nd, key):
@@ -349,12 +435,15 @@ def product_namespace():
     from neurodiffeq_b200 import operators as ops
     from neurodiffeq_b200.networks import FCNN, SinActv, Resnet
     from neurodiffeq_b200 import conditions as c
+    from neurodiffeq_b200 import function_basis as fb
     return types.SimpleNamespace(
         diff=diff, FCNN=FCNN, Resnet=Resnet, SinActv=SinActv, IVP=c.IVP, BundleIVP=c.BundleIVP, DirichletBVP2D=c.DirichletBVP2D,
         IBVP1D=c.IBVP1D, DirichletBVPSpherical=c.DirichletBVPSpherical, NoCondition=c.NoCondition,
         DoubleEndedBVP1D=c.DoubleEndedBVP1D, EnsembleCondition=c.EnsembleCondition,
         spherical_laplacian=ops.spherical_laplacian, laplacian=ops.laplacian, grad=ops.grad, div=ops.div,
-        curl=ops.curl)
+        curl=ops.curl, DirichletBVPSphericalBasis=c.DirichletBVPSphericalBasis,
+        InfDirichletBVPSphericalBasis=c.InfDirichletBVPSphericalBasis, HarmonicsLaplacian=fb.HarmonicsLaplacian,
+        RealSphericalHarmonics=fb.RealSphericalHarmonics)
 
 
 def distinct(nets):
@@ -384,5 +473,5 @@ def build_fused(key, params=None, seed=0, device=None):
     nets, conds = wl.make_nets(), wl.make_conditions()
     if params is not None:
         set_params(nets, params)
-    fp = FusedProblem(nets, conds, bundle_eq_wrapper(wl), len(wl.coord_names), device=device)
+    fp = FusedProblem(nets, conds, bundle_eq_wrapper(wl), len(wl.coord_names), coords_for_condition(key), device=device)
     return wl, nets, conds, fp
