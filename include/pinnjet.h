@@ -145,6 +145,28 @@ int pj_forward_train_jit(void* cu_function, const PjSpec* spec, const int32_t* p
 int pj_backward(const PjSpec* spec, const float* const* coords, int64_t n_points, const float* theta_pack,
                 float* grad_theta /*device, accumulated*/, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- float64 (the reference's precision) --------------------------------------------------------------------------------
+ * The same entry points with double buffers: coordinates, theta, theta_pack, grad_theta, u, residuals, sum r^2, rbar and
+ * loss_scale are double; PjSpec (dir stays float: directions are 0/1 vectors) and the programs' layout are unchanged, but
+ * the programs must be the double lowering (symbolic.Program.to_f64: OP_CONST holds a double in its two operand words).
+ * Sizes and plans differ from the float ones (pj_sizes_f64, pj_plan_info_f64): FFMA-family kernels on DFMA whatever
+ * PINNJET_TC says (tc = 0), 2-point thread tiles, at most 319 forward CTAs (their double loss partials fit below the
+ * ticket: the first 4 KB of the workspace must still be zero before the first call).  There is no f64 specialised
+ * kernel and no f64 fused all-reduce. */
+int pj_sizes_f64(const PjSpec* spec, int64_t n_points, PjSizes* out);
+int pj_plan_info_f64(const PjSpec* spec, int64_t n_points, int64_t* out, int32_t n_out);
+int pj_pack_f64(const PjSpec* spec, const double* theta, double* theta_pack, void* stream);
+int pj_pack_zero_f64(const PjSpec* spec, const double* theta, double* theta_pack, double* zero_buf, int64_t n_zero, void* stream);
+int pj_forward_f64(const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w, int32_t prog_w_len,
+                   const double* const* coords, int64_t n_points, const double* theta_pack, double* u_out, double* resid_out,
+                   double* sumsq_out, void* workspace, size_t workspace_bytes, void* stream);
+int pj_forward_train_f64(const PjSpec* spec, const int32_t* prog_train, int32_t prog_len, const int32_t* prog_w,
+                         int32_t prog_w_len, const double* const* coords, int64_t n_points, const double* theta_pack,
+                         double loss_scale, const double* rbar, double* resid_out, double* sumsq_out, void* workspace,
+                         size_t workspace_bytes, void* stream);
+int pj_backward_f64(const PjSpec* spec, const double* const* coords, int64_t n_points, const double* theta_pack,
+                    double* grad_theta, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- data parallelism (SURVEY.md 8e): the one collective of the path -------------------------------------------------
  * Replaces nothing in the reference (single process); replaces the NCCL all-reduce of the flat gradient buffer.  Every rank passes the device
  * addresses of ONE symmetric buffer per rank (pj_allreduce_bytes(n) bytes each, zero-initialised before the first call,

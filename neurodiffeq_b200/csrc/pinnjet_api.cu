@@ -14,10 +14,13 @@
 namespace pj {
 
 // per-scheme launchers and occupancy query, defined in pinnjet_inst.cu (one translation unit per jet-channel scheme)
-#define PJ_DECL(N1, N2, WL)                                                                        \
-    cudaError_t launch_k1_##N1##_##N2##_##WL(const K1Args& a, int grid, int smem, cudaStream_t s); \
-    cudaError_t launch_k2_##N1##_##N2##_##WL(const K2Args& a, int grid, int smem, cudaStream_t s); \
-    int occupancy_##N1##_##N2##_##WL(const Plan& pl, int k, int smem);
+#define PJ_DECL(N1, N2, WL)                                                                               \
+    cudaError_t launch_k1_##N1##_##N2##_##WL(const K1Args& a, int grid, int smem, cudaStream_t s);        \
+    cudaError_t launch_k2_##N1##_##N2##_##WL(const K2Args& a, int grid, int smem, cudaStream_t s);        \
+    int occupancy_##N1##_##N2##_##WL(const Plan& pl, int k, int smem);                                    \
+    cudaError_t launch_k1_f64_##N1##_##N2##_##WL(const K1ArgsF64& a, int grid, int smem, cudaStream_t s); \
+    cudaError_t launch_k2_f64_##N1##_##N2##_##WL(const K2ArgsF64& a, int grid, int smem, cudaStream_t s); \
+    int occupancy_f64_##N1##_##N2##_##WL(const Plan& pl, int k, int smem);
 PJ_DECL(1, 0, 0)
 PJ_DECL(1, 1, 0)
 PJ_DECL(2, 0, 0)
@@ -30,18 +33,32 @@ PJ_DECL(3, 1, 3)
 PJ_DECL(4, 1, 4)   // 4 directions (e.g. x, t, a boundary abscissa and one polarisation direction), combined only
 #undef PJ_DECL
 cudaError_t launch_reduce(const float* gpart, int n_parts, long long n_theta, float* grad, cudaStream_t s);
+cudaError_t launch_reduce_f64(const double* gpart, int n_parts, long long n_theta, double* grad, cudaStream_t s);
 cudaError_t launch_reduce_allreduce(const unsigned long long* peers, int rank, int world, const float* gpart, int n_parts,
                                     long long n_theta, float* buf, long long n, cudaStream_t s);   // pinnjet_comm.cu
 
-typedef cudaError_t (*K1Launch)(const K1Args&, int, int, cudaStream_t);
-typedef cudaError_t (*K2Launch)(const K2Args&, int, int, cudaStream_t);
-struct SchemeEntry {
-    int n1, n2, wl;
-    K1Launch k1;
-    K2Launch k2;
+template <typename R> struct Kernels;   // the launchers and occupancy query of one scheme for element type R
+template <> struct Kernels<float> {
+    cudaError_t (*k1)(const K1Args&, int, int, cudaStream_t);
+    cudaError_t (*k2)(const K2Args&, int, int, cudaStream_t);
     int (*occ)(const Plan&, int, int);
 };
-#define PJ_ENTRY(N1, N2, WL) {N1, N2, WL, launch_k1_##N1##_##N2##_##WL, launch_k2_##N1##_##N2##_##WL, occupancy_##N1##_##N2##_##WL}
+template <> struct Kernels<double> {
+    cudaError_t (*k1)(const K1ArgsF64&, int, int, cudaStream_t);
+    cudaError_t (*k2)(const K2ArgsF64&, int, int, cudaStream_t);
+    int (*occ)(const Plan&, int, int);
+};
+struct SchemeEntry {
+    int n1, n2, wl;
+    Kernels<float> f32;
+    Kernels<double> f64;
+    template <typename R> const Kernels<R>& of() const;
+};
+template <> const Kernels<float>& SchemeEntry::of<float>() const { return f32; }
+template <> const Kernels<double>& SchemeEntry::of<double>() const { return f64; }
+#define PJ_ENTRY(N1, N2, WL)                                                                                                  \
+    {N1, N2, WL, {launch_k1_##N1##_##N2##_##WL, launch_k2_##N1##_##N2##_##WL, occupancy_##N1##_##N2##_##WL},                   \
+     {launch_k1_f64_##N1##_##N2##_##WL, launch_k2_f64_##N1##_##N2##_##WL, occupancy_f64_##N1##_##N2##_##WL}}
 static const SchemeEntry kSchemes[] = {
     PJ_ENTRY(1, 0, 0), PJ_ENTRY(1, 1, 0), PJ_ENTRY(2, 0, 0), PJ_ENTRY(2, 1, 0), PJ_ENTRY(2, 2, 0),
     PJ_ENTRY(3, 0, 0), PJ_ENTRY(3, 3, 0), PJ_ENTRY(2, 1, 2), PJ_ENTRY(3, 1, 3), PJ_ENTRY(4, 1, 4),
@@ -70,18 +87,22 @@ static const SchemeEntry* find_scheme(int n1, int n2, int wl) {
 #define PJ_TC_DEFAULT 0
 #endif
 
-static int occupancy(const PjSpec& sp, const Plan& pl, int k, int smem) { return find_scheme(sp.n1, sp.n2, sp.wl)->occ(pl, k, smem); }
+template <typename R>
+static int occupancy(const PjSpec& sp, const Plan& pl, int k, int smem) {
+    return find_scheme(sp.n1, sp.n2, sp.wl)->of<R>().occ(pl, k, smem);
+}
 
-// make_plan (pinnjet_plan.cpp) for the current device and the current value of PINNJET_TC
+// make_plan (pinnjet_plan.cpp) for the current device, the current value of PINNJET_TC and the kernels of element type R
+template <typename R = float>
 static int device_plan(const PjSpec& sp, long long N, int prog_len, Plan& pl, int prog_w_len = 0) {
     if (!find_scheme(sp.n1, sp.n2, sp.wl))
         return fail(-2, "jet channel scheme (n1=%d, n2=%d, wl=%d) has no compiled kernel", sp.n1, sp.n2, sp.wl);
-    PlanDevice dev = {0, PJ_TC_DEFAULT, occupancy};
+    PlanDevice dev = {0, PJ_TC_DEFAULT, occupancy<R>};
     int d = 0;
     if (cudaGetDevice(&d) != cudaSuccess || cudaDeviceGetAttribute(&dev.sms, cudaDevAttrMultiProcessorCount, d) != cudaSuccess)
         return fail(-4, "cannot query the CUDA device");
     if (const char* env = getenv("PINNJET_TC")) dev.tc_level = (env[0] >= '0' && env[0] <= '2' && env[1] == 0) ? env[0] - '0' : 0;
-    return make_plan(sp, N, prog_len, prog_w_len, dev, pl, g_err, (int)sizeof(g_err));
+    return make_plan(sp, N, prog_len, prog_w_len, dev, pl, g_err, (int)sizeof(g_err), (int)sizeof(R));
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -112,8 +133,9 @@ __device__ void pack_bf16x3_image(unsigned char* img, const float* W, int rows, 
 // zero_buf[0, n_zero) when given (pj_pack_zero: the optimizer.zero_grad() of the step rides along instead of a fill launch).
 constexpr int PACK_PARTS = 4;
 
-__global__ void pack_kernel(const __grid_constant__ PackArgs A, const float* __restrict__ theta, float* __restrict__ pack,
-                            float* __restrict__ zero_buf, long long n_zero) {
+template <typename R>
+__global__ void pack_kernel(const __grid_constant__ PackArgs A, const R* __restrict__ theta, R* __restrict__ pack,
+                            R* __restrict__ zero_buf, long long n_zero) {
     const PjSpec& sp = A.spec;
     const Plan& pl = A.plan;
     pdl_launch_dependents();   // the forward kernel's CTAs may become resident now; they wait for this grid before reading `pack`
@@ -129,55 +151,59 @@ __global__ void pack_kernel(const __grid_constant__ PackArgs A, const float* __r
     const int L = net.n_linear - 1;
     if (l > L) return;
     const int fin = net.width[l], fout = net.width[l + 1];
-    const float* W = theta + net.w_off[l];
-    const float* b = theta + net.b_off[l];
+    const R* W = theta + net.w_off[l];
+    const R* b = theta + net.b_off[l];
     const int tid = threadIdx.x + part * blockDim.x, nt = blockDim.x * nparts;   // this block's share of every loop
     if (l == 0) {
         const int hp1 = pl.hp[n][1];
-        float* wt = pack + pl.s_wt0[n];
+        R* wt = pack + pl.s_wt0[n];
         for (int e = tid; e < fin * hp1; e += nt) {
             const int i = e / hp1, u = e - i * hp1;
             wt[e] = (u < fout) ? W[u * fin + i] : 0.0f;
         }
-        float* bp = pack + pl.s_b[n][0];
+        R* bp = pack + pl.s_b[n][0];
         for (int u = tid; u < hp1; u += nt) bp[u] = (u < fout) ? b[u] : 0.0f;
-        float* dz = pack + pl.s_dz[n];   // first-order channel seeds of layer 1: W0 . dir_f (same for every point)
+        R* dz = pack + pl.s_dz[n];   // first-order channel seeds of layer 1: W0 . dir_f (same for every point)
         for (int e = tid; e < PJ_MAX_DIRS * hp1; e += nt) {
             const int f = e / hp1, u = e - f * hp1;
-            float v = 0.0f;
+            R v = 0.0f;
             if (u < fout && f < sp.n1)
-                for (int i = 0; i < fin; ++i) v = fmaf(W[u * fin + i], sp.dir[f][net.in_coord[i]], v);
+                for (int i = 0; i < fin; ++i) v = fma(W[u * fin + i], R(sp.dir[f][net.in_coord[i]]), v);
             dz[e] = v;
         }
     }
     if (l >= 1 && l < L) {
         const int hi = pl.hp[n][l], ho = pl.hp[n][l + 1];
-        float* wt = pack + pl.b_wt[n][l];
-        float* wo = pack + pl.b_wo[n][l];
+        R* wt = pack + pl.b_wt[n][l];
+        R* wo = pack + pl.b_wo[n][l];
         for (int e = tid; e < hi * ho; e += nt) {
             const int i = e / ho, u = e - i * ho;              // K-major [in][out]
             wt[e] = (i < fin && u < fout) ? W[u * fin + i] : 0.0f;
             const int u2 = e / hi, i2 = e - u2 * hi;           // out-major [out][in]
             wo[e] = (i2 < fin && u2 < fout) ? W[u2 * fin + i2] : 0.0f;
         }
-        float* bp = pack + pl.s_b[n][l];
+        R* bp = pack + pl.s_b[n][l];
         for (int u = tid; u < ho; u += nt) bp[u] = (u < fout) ? b[u] : 0.0f;
-        if (hi == TC_H && ho == TC_H) pack_bf16x3_image(reinterpret_cast<unsigned char*>(pack + pl.b_wimg[n][l]), W, TC_H, fout, fin, tid, nt);
+        if constexpr (sizeof(R) == 4) {   // the tensor-core kernels are float only
+            if (hi == TC_H && ho == TC_H) pack_bf16x3_image(reinterpret_cast<unsigned char*>(pack + pl.b_wimg[n][l]), W, TC_H, fout, fin, tid, nt);
+        }
     }
     if (l == L) {
         const int hpL = pl.hp[n][L];
-        float* wlt = pack + pl.s_wlt[n];
-        float* wlo = pack + pl.s_wlo[n];
+        R* wlt = pack + pl.s_wlt[n];
+        R* wlo = pack + pl.s_wlo[n];
         for (int e = tid; e < hpL * fout; e += nt) {
             const int k = e / fout, o = e - k * fout;
             wlt[e] = (k < fin) ? W[o * fin + k] : 0.0f;
             const int o2 = e / hpL, k2 = e - o2 * hpL;
             wlo[e] = (k2 < fin) ? W[o2 * fin + k2] : 0.0f;
         }
-        float* bo = pack + pl.s_bout[n];
+        R* bo = pack + pl.s_bout[n];
         for (int o = tid; o < (fout + 3) / 4 * 4; o += nt) bo[o] = (o < fout) ? b[o] : 0.0f;   // region padded to 4
-        if (hpL == TC_H && fout <= 4)   // rows = outputs (zero padded to 16), K = hidden unit: nets the tensor cores can take
-            pack_bf16x3_image(reinterpret_cast<unsigned char*>(pack + pl.b_woutimg[n]), W, 16, fout, fin, tid, nt);
+        if constexpr (sizeof(R) == 4) {
+            if (hpL == TC_H && fout <= 4)   // rows = outputs (zero padded to 16), K = hidden unit: nets the tensor cores can take
+                pack_bf16x3_image(reinterpret_cast<unsigned char*>(pack + pl.b_woutimg[n]), W, 16, fout, fin, tid, nt);
+        }
     }
 }
 
@@ -196,11 +222,15 @@ int pj_abi_version(void) { return PJ_ABI_VERSION; }
 
 const char* pj_last_error(void) { return g_err; }
 
-int pj_sizes(const PjSpec* spec, int64_t n_points, PjSizes* out) {
+}  // extern "C"
+
+// Each entry point and its _f64 twin share one body, templated on the element type R of the buffers.
+template <typename R>
+static int sizes_impl(const PjSpec* spec, int64_t n_points, PjSizes* out) {
     if (!spec || !out) return fail(-1, "null argument");
     Plan pl;
-    if (int rc = device_plan(*spec, n_points, 0, pl)) return rc;
-    out->pack_bytes = pl.pack_floats * 4;
+    if (int rc = device_plan<R>(*spec, n_points, 0, pl)) return rc;
+    out->pack_bytes = pl.pack_floats * (int64_t)sizeof(R);
     out->workspace_bytes = pl.ws_bytes;
     out->tile_points = pl.T;
     out->grid = pl.grid;
@@ -211,10 +241,11 @@ int pj_sizes(const PjSpec* spec, int64_t n_points, PjSizes* out) {
     return 0;
 }
 
-int pj_plan_info(const PjSpec* spec, int64_t n_points, int64_t* out, int32_t n_out) {
+template <typename R>
+static int plan_info_impl(const PjSpec* spec, int64_t n_points, int64_t* out, int32_t n_out) {
     if (!spec || !out) return fail(-1, "null argument");
     Plan pl;
-    if (int rc = device_plan(*spec, n_points, 0, pl)) return rc;
+    if (int rc = device_plan<R>(*spec, n_points, 0, pl)) return rc;
     const long long head[19] = {pl.T, pl.P, pl.Q, pl.C, pl.RS, pl.n_tiles, pl.grid, pl.hmax, pl.n_stage, pl.n_stage_bwd,
                                 pl.resident_fwd, pl.resident_bwd, pl.zj_tile_floats, pl.ws_zj, pl.ws_seed, pl.ws_gpart,
                                 pl.ws_bytes, pl.k1_bytes, pl.k2_bytes};
@@ -229,22 +260,46 @@ int pj_plan_info(const PjSpec* spec, int64_t n_points, int64_t* out, int32_t n_o
     return 0;
 }
 
-static int pack_impl(const PjSpec* spec, const float* theta, float* theta_pack, float* zero_buf, long long n_zero, void* stream) {
+template <typename R>
+static int pack_impl(const PjSpec* spec, const R* theta, R* theta_pack, R* zero_buf, long long n_zero, void* stream) {
     if (!spec || !theta || !theta_pack) return fail(-1, "null argument");
     PackArgs a;
     a.spec = *spec;
-    if (int rc = device_plan(*spec, 1, 0, a.plan)) return rc;
-    pack_kernel<<<dim3(spec->n_nets * PJ_MAX_LINEAR, PACK_PARTS), 256, 0, (cudaStream_t)stream>>>(a, theta, theta_pack, zero_buf, n_zero);
+    if (int rc = device_plan<R>(*spec, 1, 0, a.plan)) return rc;
+    pack_kernel<R><<<dim3(spec->n_nets * PJ_MAX_LINEAR, PACK_PARTS), 256, 0, (cudaStream_t)stream>>>(a, theta, theta_pack, zero_buf, n_zero);
     return check_cuda(cudaGetLastError(), "pack launch");
 }
 
+template <typename R>
+static int pack_zero_impl(const PjSpec* spec, const R* theta, R* theta_pack, R* zero_buf, int64_t n_zero, void* stream) {
+    if (!zero_buf || n_zero < 1) return fail(-1, "pj_pack_zero: nothing to clear");
+    return pack_impl(spec, theta, theta_pack, zero_buf, n_zero, stream);
+}
+
+extern "C" {
+
+int pj_sizes(const PjSpec* spec, int64_t n_points, PjSizes* out) { return sizes_impl<float>(spec, n_points, out); }
+int pj_sizes_f64(const PjSpec* spec, int64_t n_points, PjSizes* out) { return sizes_impl<double>(spec, n_points, out); }
+
+int pj_plan_info(const PjSpec* spec, int64_t n_points, int64_t* out, int32_t n_out) {
+    return plan_info_impl<float>(spec, n_points, out, n_out);
+}
+int pj_plan_info_f64(const PjSpec* spec, int64_t n_points, int64_t* out, int32_t n_out) {
+    return plan_info_impl<double>(spec, n_points, out, n_out);
+}
+
 int pj_pack(const PjSpec* spec, const float* theta, float* theta_pack, void* stream) {
-    return pack_impl(spec, theta, theta_pack, nullptr, 0, stream);
+    return pack_impl<float>(spec, theta, theta_pack, nullptr, 0, stream);
+}
+int pj_pack_f64(const PjSpec* spec, const double* theta, double* theta_pack, void* stream) {
+    return pack_impl<double>(spec, theta, theta_pack, nullptr, 0, stream);
 }
 
 int pj_pack_zero(const PjSpec* spec, const float* theta, float* theta_pack, float* zero_buf, int64_t n_zero, void* stream) {
-    if (!zero_buf || n_zero < 1) return fail(-1, "pj_pack_zero: nothing to clear");
-    return pack_impl(spec, theta, theta_pack, zero_buf, n_zero, stream);
+    return pack_zero_impl(spec, theta, theta_pack, zero_buf, n_zero, stream);
+}
+int pj_pack_zero_f64(const PjSpec* spec, const double* theta, double* theta_pack, double* zero_buf, int64_t n_zero, void* stream) {
+    return pack_zero_impl(spec, theta, theta_pack, zero_buf, n_zero, stream);
 }
 
 // The specialised forward kernel (neurodiffeq_b200/jit.py) arrives as a CUfunction handle of a module the caller loaded:
@@ -260,17 +315,24 @@ static CuLaunchKernelEx cu_launch_kernel_ex() {
     return fn;
 }
 
+}  // extern "C"
+
+template <typename R> struct ArgsOf;
+template <> struct ArgsOf<float> { typedef K1Args K1; typedef K2Args K2; };
+template <> struct ArgsOf<double> { typedef K1ArgsF64 K1; typedef K2ArgsF64 K2; };
+
+template <typename R>
 static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, const int32_t* prog_w, int32_t prog_w_len,
-                  const float* const* coords, int64_t n,
-                  const float* theta_pack, int mode, float loss_scale, const float* rbar, float* u_out, float* r_out,
-                  float* sumsq_out, void* ws, size_t ws_bytes, void* stream, void* jit_function = nullptr) {
+                  const R* const* coords, int64_t n,
+                  const R* theta_pack, int mode, R loss_scale, const R* rbar, R* u_out, R* r_out,
+                  R* sumsq_out, void* ws, size_t ws_bytes, void* stream, void* jit_function = nullptr) {
     if (!spec || !prog || !coords || !theta_pack || !ws) return fail(-1, "null argument");
-    K1Args a;
+    typename ArgsOf<R>::K1 a;
     memset(&a, 0, sizeof(a));
     a.spec = *spec;
     if (spec->wl > 0 && (!prog_w || prog_w_len < 1)) return fail(-1, "spec->wl=%d needs a weight program", spec->wl);
     if (spec->wl == 0) prog_w_len = 0;
-    if (int rc = device_plan(*spec, n, prog_len, a.plan, prog_w_len)) return rc;
+    if (int rc = device_plan<R>(*spec, n, prog_len, a.plan, prog_w_len)) return rc;
     const size_t need = mode == 1 ? (size_t)a.plan.ws_bytes : (size_t)LOSS_PART_BYTES;
     if (ws_bytes < need) return fail(-1, "workspace too small: %zu < %zu bytes", ws_bytes, need);
     if (a.plan.k1_bytes > SMEM_LIMIT) return fail(-2, "forward kernel needs %d B of shared memory", a.plan.k1_bytes);
@@ -290,13 +352,13 @@ static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, con
     a.u_out = u_out;
     a.r_out = r_out;
     char* w = static_cast<char*>(ws);
-    a.loss_part = reinterpret_cast<float*>(w + a.plan.ws_loss);
-    a.dbg = a.loss_part + LOSS_DBG_WORD;
-    a.ticket = reinterpret_cast<unsigned*>(a.loss_part + LOSS_TICKET_WORD);
+    a.loss_part = reinterpret_cast<R*>(w + a.plan.ws_loss);
+    a.dbg = reinterpret_cast<float*>(w + a.plan.ws_loss) + LOSS_DBG_WORD;
+    a.ticket = reinterpret_cast<unsigned*>(w + a.plan.ws_loss) + LOSS_TICKET_WORD;
     a.sumsq_out = sumsq_out;
-    a.zj = mode == 1 ? reinterpret_cast<float*>(w + (a.plan.tc ? a.plan.ws_tcrec : a.plan.ws_zj)) : nullptr;
-    a.seeds = mode == 1 ? reinterpret_cast<float*>(w + a.plan.ws_seed) : nullptr;
-    a.wts = mode == 1 ? reinterpret_cast<float*>(w + a.plan.ws_wts) : nullptr;
+    a.zj = mode == 1 ? reinterpret_cast<R*>(w + (a.plan.tc ? a.plan.ws_tcrec : a.plan.ws_zj)) : nullptr;
+    a.seeds = mode == 1 ? reinterpret_cast<R*>(w + a.plan.ws_seed) : nullptr;
+    a.wts = mode == 1 ? reinterpret_cast<R*>(w + a.plan.ws_wts) : nullptr;
     const SchemeEntry* e = find_scheme(spec->n1, spec->n2, spec->wl);
     if (jit_function) {   // the problem's own forward kernel: same arguments, same plan
         if (!a.plan.tc) return fail(-2, "the specialised forward kernel exists for the tensor-core path only");
@@ -321,30 +383,45 @@ static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, con
         if (rc != 0) return fail(-5, "cuLaunchKernelEx of the specialised forward kernel failed (%d)", rc);
         return 0;
     }
-    return check_cuda(e->k1(a, a.plan.grid, a.plan.k1_bytes, (cudaStream_t)stream), "forward launch");
+    return check_cuda(e->of<R>().k1(a, a.plan.grid, a.plan.k1_bytes, (cudaStream_t)stream), "forward launch");
 }
+
+extern "C" {
 
 int pj_forward(const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w, int32_t prog_w_len,
                const float* const* coords, int64_t n_points, const float* theta_pack, float* u_out, float* resid_out,
                float* sumsq_out, void* workspace, size_t workspace_bytes, void* stream) {
-    return run_k1(spec, prog_eval, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 0, 0.0f, nullptr, u_out, resid_out, sumsq_out,
-                  workspace, workspace_bytes, stream);
+    return run_k1<float>(spec, prog_eval, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 0, 0.0f, nullptr, u_out, resid_out,
+                         sumsq_out, workspace, workspace_bytes, stream);
+}
+int pj_forward_f64(const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w, int32_t prog_w_len,
+                   const double* const* coords, int64_t n_points, const double* theta_pack, double* u_out, double* resid_out,
+                   double* sumsq_out, void* workspace, size_t workspace_bytes, void* stream) {
+    return run_k1<double>(spec, prog_eval, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 0, 0.0, nullptr, u_out, resid_out,
+                          sumsq_out, workspace, workspace_bytes, stream);
 }
 
 int pj_forward_train(const PjSpec* spec, const int32_t* prog_train, int32_t prog_len, const int32_t* prog_w,
                      int32_t prog_w_len, const float* const* coords, int64_t n_points, const float* theta_pack,
                      float loss_scale, const float* rbar, float* resid_out, float* sumsq_out, void* workspace,
                      size_t workspace_bytes, void* stream) {
-    return run_k1(spec, prog_train, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 1, loss_scale, rbar, nullptr, resid_out,
-                  sumsq_out, workspace, workspace_bytes, stream);
+    return run_k1<float>(spec, prog_train, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 1, loss_scale, rbar, nullptr,
+                         resid_out, sumsq_out, workspace, workspace_bytes, stream);
+}
+int pj_forward_train_f64(const PjSpec* spec, const int32_t* prog_train, int32_t prog_len, const int32_t* prog_w,
+                         int32_t prog_w_len, const double* const* coords, int64_t n_points, const double* theta_pack,
+                         double loss_scale, const double* rbar, double* resid_out, double* sumsq_out, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+    return run_k1<double>(spec, prog_train, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 1, loss_scale, rbar, nullptr,
+                          resid_out, sumsq_out, workspace, workspace_bytes, stream);
 }
 
 int pj_forward_jit(void* cu_function, const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w,
                    int32_t prog_w_len, const float* const* coords, int64_t n_points, const float* theta_pack, float* u_out,
                    float* resid_out, float* sumsq_out, void* workspace, size_t workspace_bytes, void* stream) {
     if (!cu_function) return fail(-1, "null kernel handle");
-    return run_k1(spec, prog_eval, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 0, 0.0f, nullptr, u_out, resid_out, sumsq_out,
-                  workspace, workspace_bytes, stream, cu_function);
+    return run_k1<float>(spec, prog_eval, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 0, 0.0f, nullptr, u_out, resid_out,
+                         sumsq_out, workspace, workspace_bytes, stream, cu_function);
 }
 
 int pj_forward_train_jit(void* cu_function, const PjSpec* spec, const int32_t* prog_train, int32_t prog_len, const int32_t* prog_w,
@@ -352,18 +429,21 @@ int pj_forward_train_jit(void* cu_function, const PjSpec* spec, const int32_t* p
                          float loss_scale, float* resid_out, float* sumsq_out, void* workspace, size_t workspace_bytes,
                          void* stream) {
     if (!cu_function) return fail(-1, "null kernel handle");
-    return run_k1(spec, prog_train, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 1, loss_scale, nullptr, nullptr, resid_out,
-                  sumsq_out, workspace, workspace_bytes, stream, cu_function);
+    return run_k1<float>(spec, prog_train, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 1, loss_scale, nullptr, nullptr,
+                         resid_out, sumsq_out, workspace, workspace_bytes, stream, cu_function);
 }
 
+}  // extern "C"
+
 // K2 on the records / seeds pj_forward_train left in the workspace; the per-CTA gradient partials stay in the workspace
-static int run_k2(const PjSpec* spec, const float* const* coords, int64_t n_points, const float* theta_pack, void* workspace,
-                  size_t workspace_bytes, void* stream, const float** gpart, int* n_parts) {
+template <typename R>
+static int run_k2(const PjSpec* spec, const R* const* coords, int64_t n_points, const R* theta_pack, void* workspace,
+                  size_t workspace_bytes, void* stream, const R** gpart, int* n_parts) {
     if (!spec || !coords || !theta_pack || !workspace) return fail(-1, "null argument");
-    K2Args a;
+    typename ArgsOf<R>::K2 a;
     memset(&a, 0, sizeof(a));
     a.spec = *spec;
-    if (int rc = device_plan(*spec, n_points, 0, a.plan)) return rc;
+    if (int rc = device_plan<R>(*spec, n_points, 0, a.plan)) return rc;
     if (workspace_bytes < (size_t)a.plan.ws_bytes)
         return fail(-1, "workspace too small: %zu < %lld bytes", workspace_bytes, a.plan.ws_bytes);
     if (a.plan.k2_bytes > SMEM_LIMIT) return fail(-2, "backward kernel needs %d B of shared memory", a.plan.k2_bytes);
@@ -371,25 +451,44 @@ static int run_k2(const PjSpec* spec, const float* const* coords, int64_t n_poin
     a.pack = theta_pack;
     a.N = n_points;
     char* w = static_cast<char*>(workspace);
-    a.zj = reinterpret_cast<const float*>(w + (a.plan.tc ? a.plan.ws_tcrec : a.plan.ws_zj));
-    a.seeds = reinterpret_cast<const float*>(w + a.plan.ws_seed);
-    a.gpart = reinterpret_cast<float*>(w + a.plan.ws_gpart);
-    a.wts = reinterpret_cast<const float*>(w + a.plan.ws_wts);
+    a.zj = reinterpret_cast<const R*>(w + (a.plan.tc ? a.plan.ws_tcrec : a.plan.ws_zj));
+    a.seeds = reinterpret_cast<const R*>(w + a.plan.ws_seed);
+    a.gpart = reinterpret_cast<R*>(w + a.plan.ws_gpart);
+    a.wts = reinterpret_cast<const R*>(w + a.plan.ws_wts);
     a.dbg = reinterpret_cast<float*>(w + a.plan.ws_loss) + LOSS_DBG_WORD;
     const SchemeEntry* e = find_scheme(spec->n1, spec->n2, spec->wl);
-    if (int rc = check_cuda(e->k2(a, a.plan.grid_bwd, a.plan.k2_bytes, (cudaStream_t)stream), "backward launch")) return rc;
+    if (int rc = check_cuda(e->of<R>().k2(a, a.plan.grid_bwd, a.plan.k2_bytes, (cudaStream_t)stream), "backward launch")) return rc;
     *gpart = a.gpart;
     *n_parts = a.plan.grid_bwd;
     return 0;
 }
 
-int pj_backward(const PjSpec* spec, const float* const* coords, int64_t n_points, const float* theta_pack,
-                float* grad_theta, void* workspace, size_t workspace_bytes, void* stream) {
+static cudaError_t reduce(const float* gpart, int n_parts, long long n_theta, float* grad, cudaStream_t s) {
+    return launch_reduce(gpart, n_parts, n_theta, grad, s);
+}
+static cudaError_t reduce(const double* gpart, int n_parts, long long n_theta, double* grad, cudaStream_t s) {
+    return launch_reduce_f64(gpart, n_parts, n_theta, grad, s);
+}
+
+template <typename R>
+static int backward_impl(const PjSpec* spec, const R* const* coords, int64_t n_points, const R* theta_pack, R* grad_theta,
+                         void* workspace, size_t workspace_bytes, void* stream) {
     if (!grad_theta) return fail(-1, "null argument");
-    const float* gpart = nullptr;
+    const R* gpart = nullptr;
     int n_parts = 0;
     if (int rc = run_k2(spec, coords, n_points, theta_pack, workspace, workspace_bytes, stream, &gpart, &n_parts)) return rc;
-    return check_cuda(launch_reduce(gpart, n_parts, spec->n_theta, grad_theta, (cudaStream_t)stream), "reduce launch");
+    return check_cuda(reduce(gpart, n_parts, spec->n_theta, grad_theta, (cudaStream_t)stream), "reduce launch");
+}
+
+extern "C" {
+
+int pj_backward(const PjSpec* spec, const float* const* coords, int64_t n_points, const float* theta_pack,
+                float* grad_theta, void* workspace, size_t workspace_bytes, void* stream) {
+    return backward_impl(spec, coords, n_points, theta_pack, grad_theta, workspace, workspace_bytes, stream);
+}
+int pj_backward_f64(const PjSpec* spec, const double* const* coords, int64_t n_points, const double* theta_pack,
+                    double* grad_theta, void* workspace, size_t workspace_bytes, void* stream) {
+    return backward_impl(spec, coords, n_points, theta_pack, grad_theta, workspace, workspace_bytes, stream);
 }
 
 int pj_backward_allreduce(const PjSpec* spec, const float* const* coords, int64_t n_points, const float* theta_pack,
@@ -400,7 +499,7 @@ int pj_backward_allreduce(const PjSpec* spec, const float* const* coords, int64_
         return fail(-1, "rank %d / world %d / n_tail %lld out of range", rank, world, (long long)n_tail);
     const float* gpart = nullptr;
     int n_parts = 0;
-    if (int rc = run_k2(spec, coords, n_points, theta_pack, workspace, workspace_bytes, stream, &gpart, &n_parts)) return rc;
+    if (int rc = run_k2<float>(spec, coords, n_points, theta_pack, workspace, workspace_bytes, stream, &gpart, &n_parts)) return rc;
     return check_cuda(launch_reduce_allreduce(reinterpret_cast<const unsigned long long*>(peer_buffers), rank, world, gpart, n_parts,
                                               spec->n_theta, gradbuf, spec->n_theta + n_tail, (cudaStream_t)stream),
                       "reduce + all-reduce launch");

@@ -52,45 +52,52 @@ inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, 
 enum : int {
     OP_CONST = 0, OP_COORD, OP_NET, OP_RBAR, OP_PARAM, OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_NEG, OP_SIN, OP_COS, OP_EXP,
     OP_LOG, OP_TANH, OP_SQRT, OP_ABS, OP_SIGN, OP_POWC, OP_RCP, OP_ST_U, OP_ST_R, OP_ST_SEED, OP_TAN, OP_SINH, OP_COSH,
-    OP_ATAN, OP_ERF, OP_ST_W
+    OP_ATAN, OP_ERF, OP_ST_W, OP_POW   // OP_POW: double programs only
 };
 
-struct K1Args {
+// Kernel arguments for element type R (float, or double for the PJ_F64 instances of the FFMA kernels).
+template <typename R>
+struct K1ArgsT {
     PjSpec spec;
     Plan plan;
-    const float* coords[PJ_MAX_COORDS];
-    const float* pack;
+    const R* coords[PJ_MAX_COORDS];
+    const R* pack;
     const int4* prog;
     int prog_len;
     const int4* prog_w;
     int prog_w_len;
     int mode;                            // 0 = eval (u, residual), 1 = train (residual, seeds, z-jets)
     long long N;
-    float loss_scale;
-    const float* rbar;
-    float* u_out;
-    float* r_out;
-    float* zj;                           // z-jet records (tensor-core layout when plan.tc)
-    float* seeds;
-    float* wts;
-    float* loss_part;
+    R loss_scale;
+    const R* rbar;
+    R* u_out;
+    R* r_out;
+    R* zj;                               // z-jet records (tensor-core layout when plan.tc)
+    R* seeds;
+    R* wts;
+    R* loss_part;
     float* dbg;                          // diagnostic builds only (PJ_TIMING): phase cycle counters
-    float* sumsq_out;                    // non-null: the LAST warp to deliver its partial folds them all into *sumsq_out (+=)
+    R* sumsq_out;                        // non-null: the LAST warp to deliver its partial folds them all into *sumsq_out (+=)
     unsigned* ticket;                    // ... found by this counter (zero between launches; lives in the loss-partial block)
 };
 
-struct K2Args {
+template <typename R>
+struct K2ArgsT {
     PjSpec spec;
     Plan plan;
-    const float* coords[PJ_MAX_COORDS];
-    const float* pack;
+    const R* coords[PJ_MAX_COORDS];
+    const R* pack;
     long long N;
-    const float* zj;
-    const float* seeds;
-    const float* wts;
-    float* gpart;
+    const R* zj;
+    const R* seeds;
+    const R* wts;
+    R* gpart;
     float* dbg;
 };
+struct K1Args : K1ArgsT<float> {};
+struct K2Args : K2ArgsT<float> {};
+struct K1ArgsF64 : K1ArgsT<double> {};
+struct K2ArgsF64 : K2ArgsT<double> {};
 
 // ---------------------------------------------------------------------------------------------------------------------
 // PTX helpers: mbarrier, bulk TMA (cp.async.bulk -> SASS UBLKCP), named barriers, FP32 FMA on point pairs
@@ -111,7 +118,8 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // that draws the last ticket adds ALL partials to *sumsq_out and re-arms the counter.  Fixed summation order, so the result
 // is run-to-run reproducible: lane l sums partials l, l + 32, l + 64, ... in that order, then the 32 lane sums are combined
 // by an xor-shuffle tree (offsets 16, 8, 4, 2, 1).  Called by whole warps after lane 0 has written part[my index].
-__device__ __forceinline__ void fold_loss_partials(const float* part, unsigned n_parts, float* sumsq_out, unsigned* ticket, int lane) {
+template <typename R>
+__device__ __forceinline__ void fold_loss_partials(const R* part, unsigned n_parts, R* sumsq_out, unsigned* ticket, int lane) {
     if (sumsq_out == nullptr) return;
     unsigned last = 0;
     if (lane == 0) {
@@ -121,7 +129,7 @@ __device__ __forceinline__ void fold_loss_partials(const float* part, unsigned n
     last = __shfl_sync(0xffffffffu, last, 0);
     if (!last) return;
     __threadfence();
-    float s = 0.0f;
+    R s = 0.0f;
     for (unsigned p = lane; p < n_parts; p += 32) s += __ldcg(part + p);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
@@ -135,9 +143,10 @@ __device__ __forceinline__ void fold_loss_partials(const float* part, unsigned n
 // same bits: parameter i, partial group g of RED_GROUPS (contiguous ranges of the per-CTA partials, two accumulators each),
 // combined as ((g0+g1)+(g2+g3)) + ((g4+g5)+(g6+g7)).  A block handles RED_PARAMS parameters with one warp per group.
 constexpr int RED_PARAMS = 32, RED_GROUPS = 8;
-__device__ __forceinline__ float red_group_sum(const float* __restrict__ gpart, int n_parts, long long n_theta, long long i, int g) {
+template <typename R>
+__device__ __forceinline__ R red_group_sum(const R* __restrict__ gpart, int n_parts, long long n_theta, long long i, int g) {
     const int per = (n_parts + RED_GROUPS - 1) / RED_GROUPS, p_lo = g * per, p_hi = min(n_parts, p_lo + per);
-    float s0 = 0.0f, s1 = 0.0f;
+    R s0 = 0.0f, s1 = 0.0f;
     int p = p_lo;
     for (; p + 1 < p_hi; p += 2) {
         s0 += gpart[(size_t)p * n_theta + i];
@@ -146,7 +155,8 @@ __device__ __forceinline__ float red_group_sum(const float* __restrict__ gpart, 
     if (p < p_hi) s0 += gpart[(size_t)p * n_theta + i];
     return s0 + s1;
 }
-__device__ __forceinline__ float red_combine(const float (*red)[RED_PARAMS], int il) {
+template <typename R>
+__device__ __forceinline__ R red_combine(const R (*red)[RED_PARAMS], int il) {
     return ((red[0][il] + red[1][il]) + (red[2][il] + red[3][il])) + ((red[4][il] + red[5][il]) + (red[6][il] + red[7][il]));
 }
 
@@ -200,8 +210,44 @@ __device__ __forceinline__ void ffma2(f2& d, const f2 a, const f2 b) {
     const float2 x = unpack2(a), y = unpack2(b), z = unpack2(d);
     d = pack2(fmaf(x.x, y.x, z.x), fmaf(x.y, y.y, z.y));
 }
+// The double kernels' point pair: two doubles (one 16-byte shared-memory load), two DFMAs.
+struct __align__(16) d2 {
+    double x, y;
+};
+__device__ __forceinline__ d2 pack2(double x, double y) { return d2{x, y}; }
+__device__ __forceinline__ double2 unpack2(d2 v) { return make_double2(v.x, v.y); }
+__device__ __forceinline__ void ffma2(d2& d, const d2 a, const d2 b) { d = d2{fma(a.x, b.x, d.x), fma(a.y, b.y, d.y)}; }
 
-__device__ __forceinline__ float warp_sum(float v) {
+// Per element type: the point pair of the register tiles and the 16-byte unit of the weight-gradient GEMM's row loads
+// (two pairs of floats, one pair of doubles).
+template <typename R> struct Pair;
+template <> struct Pair<float> {
+    typedef f2 type;
+    typedef ulonglong2 row16;
+    __device__ static __forceinline__ void fma16(f2& d, const ulonglong2& a, const ulonglong2& b) {
+        ffma2(d, a.x, b.x);
+        ffma2(d, a.y, b.y);
+    }
+};
+template <> struct Pair<double> {
+    typedef d2 type;
+    typedef d2 row16;
+    __device__ static __forceinline__ void fma16(d2& d, const d2& a, const d2& b) { ffma2(d, a, b); }
+};
+
+// 2- and 4-element vector stores of the tile epilogues
+__device__ __forceinline__ void store2(float* p, float a, float b) { *reinterpret_cast<float2*>(p) = make_float2(a, b); }
+__device__ __forceinline__ void store2(double* p, double a, double b) { *reinterpret_cast<double2*>(p) = make_double2(a, b); }
+__device__ __forceinline__ void store4(float* p, float a, float b, float c, float d) {
+    *reinterpret_cast<float4*>(p) = make_float4(a, b, c, d);
+}
+__device__ __forceinline__ void store4(double* p, double a, double b, double c, double d) {
+    *reinterpret_cast<double2*>(p) = make_double2(a, b);
+    *reinterpret_cast<double2*>(p + 2) = make_double2(c, d);
+}
+
+template <typename R>
+__device__ __forceinline__ R warp_sum(R v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
@@ -210,9 +256,10 @@ __device__ __forceinline__ float warp_sum(float v) {
 // Reduce-scatter over the 8 point-group lanes (recursive halving): every thread contributes 8 (or 4) partial sums, lane l
 // of each 8-lane group returns the total of value l (value l >> 1 for the 4-value form, in both lanes of a pair):
 // 7 (4) shuffles instead of the 24 (12) of one butterfly all-reduce per value.
-__device__ __forceinline__ float pg_reduce_scatter8(const float (&v)[8], int pg_lane) {
+template <typename R>
+__device__ __forceinline__ R pg_reduce_scatter8(const R (&v)[8], int pg_lane) {
     const bool b2 = pg_lane & 4, b1 = pg_lane & 2, b0 = pg_lane & 1;
-    float w[4], x[2];
+    R w[4], x[2];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
         w[i] = (b2 ? v[i + 4] : v[i]) + __shfl_xor_sync(0xffffffffu, b2 ? v[i] : v[i + 4], 4);
@@ -221,13 +268,14 @@ __device__ __forceinline__ float pg_reduce_scatter8(const float (&v)[8], int pg_
         x[i] = (b1 ? w[i + 2] : w[i]) + __shfl_xor_sync(0xffffffffu, b1 ? w[i] : w[i + 2], 2);
     return (b0 ? x[1] : x[0]) + __shfl_xor_sync(0xffffffffu, b0 ? x[0] : x[1], 1);
 }
-__device__ __forceinline__ float pg_reduce_scatter4(const float (&v)[4], int pg_lane) {
+template <typename R>
+__device__ __forceinline__ R pg_reduce_scatter4(const R (&v)[4], int pg_lane) {
     const bool b2 = pg_lane & 4, b1 = pg_lane & 2;
-    float w[2];
+    R w[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i)
         w[i] = (b2 ? v[i + 2] : v[i]) + __shfl_xor_sync(0xffffffffu, b2 ? v[i] : v[i + 2], 4);
-    float x = (b1 ? w[1] : w[0]) + __shfl_xor_sync(0xffffffffu, b1 ? w[0] : w[1], 2);
+    R x = (b1 ? w[1] : w[0]) + __shfl_xor_sync(0xffffffffu, b1 ? w[0] : w[1], 2);
     return x + __shfl_xor_sync(0xffffffffu, x, 1);   // value index = pg_lane >> 1
 }
 
@@ -262,21 +310,34 @@ __device__ __forceinline__ void act_d2(int act, float z0, float& a0, float& s1, 
         s2 = -a0;
     }
 }
+// double: libdevice tanh / sincos (tanh_fast is float only)
+__device__ __forceinline__ void act_d2(int act, double z0, double& a0, double& s1, double& s2) {
+    if (act == PJ_ACT_TANH) {
+        a0 = tanh(z0);
+        s1 = fma(-a0, a0, 1.0);
+        s2 = -2.0 * a0 * s1;
+    } else {
+        sincos(z0, &a0, &s1);
+        s2 = -a0;
+    }
+}
+__device__ __forceinline__ void sincos_r(float x, float* s, float* c) { sincosf(x, s, c); }
+__device__ __forceinline__ void sincos_r(double x, double* s, double* c) { sincos(x, s, c); }
 
 // z-jet -> a-jet, in place.  WL > 0: the single second-order channel is the weighted combination L = sum_d w[d] D_d^2.
-template <int N1, int N2, int WL>
-__device__ __forceinline__ void act_forward(int act, float (&z)[1 + N1 + N2], const float* w) {
-    float a0, s1, s2;
+template <int N1, int N2, int WL, typename R>
+__device__ __forceinline__ void act_forward(int act, R (&z)[1 + N1 + N2], const R* w) {
+    R a0, s1, s2;
     act_d2(act, z[0], a0, s1, s2);
     if constexpr (WL > 0) {
         static_assert(N2 == 1, "combined mode carries one second-order channel");
-        float q = 0.0f;
+        R q = 0.0f;
 #pragma unroll
-        for (int d = 0; d < WL; ++d) q = fmaf(w[d] * z[1 + d], z[1 + d], q);
-        z[1 + N1] = fmaf(s2, q, s1 * z[1 + N1]);
+        for (int d = 0; d < WL; ++d) q = fma(w[d] * z[1 + d], z[1 + d], q);
+        z[1 + N1] = fma(s2, q, s1 * z[1 + N1]);
     } else {
 #pragma unroll
-        for (int s = 0; s < N2; ++s) z[1 + N1 + s] = fmaf(s2 * z[1 + s], z[1 + s], s1 * z[1 + N1 + s]);
+        for (int s = 0; s < N2; ++s) z[1 + N1 + s] = fma(s2 * z[1 + s], z[1 + s], s1 * z[1 + N1 + s]);
     }
 #pragma unroll
     for (int f = 0; f < N1; ++f) z[1 + f] *= s1;
@@ -286,47 +347,47 @@ __device__ __forceinline__ void act_forward(int act, float (&z)[1 + N1 + N2], co
 // reverse of the activation jet: given the stored record (channel 0 = tanh(z0) for tanh nets, z0 for sin nets; other
 // channels z-jets) and the adjoint of the a-jet, produce the a-jet (for the weight-gradient GEMM) and the adjoint of the
 // z-jet.
-template <int N1, int N2, int WL>
-__device__ __forceinline__ void act_backward(int act, const float (&z)[1 + N1 + N2], const float (&ab)[1 + N1 + N2],
-                                             float (&a)[1 + N1 + N2], float (&zb)[1 + N1 + N2], const float* w) {
-    float a0, s1, s2, s3;
+template <int N1, int N2, int WL, typename R>
+__device__ __forceinline__ void act_backward(int act, const R (&z)[1 + N1 + N2], const R (&ab)[1 + N1 + N2],
+                                             R (&a)[1 + N1 + N2], R (&zb)[1 + N1 + N2], const R* w) {
+    R a0, s1, s2, s3;
     if (act == PJ_ACT_TANH) {   // record channel 0 = tanh(z0), stored by K1: no transcendental in the reverse pass
         a0 = z[0];
-        s1 = fmaf(-a0, a0, 1.0f);
-        s2 = -2.0f * a0 * s1;
-        s3 = -2.0f * s1 * s1 - 2.0f * a0 * s2;
+        s1 = fma(-a0, a0, R(1));
+        s2 = R(-2) * a0 * s1;
+        s3 = R(-2) * s1 * s1 - R(2) * a0 * s2;
     } else {
-        sincosf(z[0], &a0, &s1);
+        sincos_r(z[0], &a0, &s1);
         s2 = -a0;
         s3 = -s1;
     }
-    float zb0 = s1 * ab[0];
+    R zb0 = s1 * ab[0];
 #pragma unroll
     for (int f = 0; f < N1; ++f) {
         zb[1 + f] = s1 * ab[1 + f];
-        zb0 = fmaf(s2 * z[1 + f], ab[1 + f], zb0);
+        zb0 = fma(s2 * z[1 + f], ab[1 + f], zb0);
         a[1 + f] = s1 * z[1 + f];
     }
     if constexpr (WL > 0) {
-        const float abL = ab[1 + N1], zL = z[1 + N1];
-        float q = 0.0f;
+        const R abL = ab[1 + N1], zL = z[1 + N1];
+        R q = 0.0f;
 #pragma unroll
         for (int d = 0; d < WL; ++d) {
-            const float wz = w[d] * z[1 + d];
-            q = fmaf(wz, z[1 + d], q);
-            zb[1 + d] = fmaf(2.0f * s2 * wz, abL, zb[1 + d]);
+            const R wz = w[d] * z[1 + d];
+            q = fma(wz, z[1 + d], q);
+            zb[1 + d] = fma(R(2) * s2 * wz, abL, zb[1 + d]);
         }
         zb[1 + N1] = s1 * abL;
-        zb0 = fmaf(fmaf(s3, q, s2 * zL), abL, zb0);
-        a[1 + N1] = fmaf(s2, q, s1 * zL);
+        zb0 = fma(fma(s3, q, s2 * zL), abL, zb0);
+        a[1 + N1] = fma(s2, q, s1 * zL);
     } else {
 #pragma unroll
         for (int s = 0; s < N2; ++s) {
-            const float zf = z[1 + s], zs = z[1 + N1 + s], abs_ = ab[1 + N1 + s];
+            const R zf = z[1 + s], zs = z[1 + N1 + s], abs_ = ab[1 + N1 + s];
             zb[1 + N1 + s] = s1 * abs_;
-            zb[1 + s] = fmaf(2.0f * s2 * zf, abs_, zb[1 + s]);
-            zb0 = fmaf(fmaf(s3 * zf, zf, s2 * zs), abs_, zb0);
-            a[1 + N1 + s] = fmaf(s2 * zf, zf, s1 * zs);
+            zb[1 + s] = fma(R(2) * s2 * zf, abs_, zb[1 + s]);
+            zb0 = fma(fma(s3 * zf, zf, s2 * zs), abs_, zb0);
+            a[1 + N1 + s] = fma(s2 * zf, zf, s1 * zs);
         }
     }
     zb[0] = zb0;
@@ -339,13 +400,14 @@ __device__ __forceinline__ void act_backward(int act, const float (&z)[1 + N1 + 
 //   B: weight chunk rows (stride ldb floats), output units contiguous                  (shared memory)
 // Thread tile P points x Q units x C channels; point pairs are packed in 64-bit register pairs.
 // ---------------------------------------------------------------------------------------------------------------------
-template <int P, int Q, int C>
-__device__ __forceinline__ void gemm_rows(f2 (&acc)[Q][C][P / 2], const float* __restrict__ a_ptr, int RS, int T,
-                                          const float* __restrict__ b_ptr, int ldb, int nrows) {
+template <int P, int Q, int C, typename R>
+__device__ __forceinline__ void gemm_rows(typename Pair<R>::type (&acc)[Q][C][P / 2], const R* __restrict__ a_ptr, int RS, int T,
+                                          const R* __restrict__ b_ptr, int ldb, int nrows) {
+    typedef typename Pair<R>::type pair;
 #pragma unroll 2
     for (int k = 0; k < nrows; ++k) {
-        f2 a[C][P / 2];
-        const float* ar = a_ptr + k * RS;
+        pair a[C][P / 2];
+        const R* ar = a_ptr + k * RS;
 #pragma unroll
         for (int c = 0; c < C; ++c) {
             if constexpr (P == 4) {
@@ -353,22 +415,31 @@ __device__ __forceinline__ void gemm_rows(f2 (&acc)[Q][C][P / 2], const float* _
                 a[c][0] = v.x;
                 a[c][1] = v.y;
             } else {
-                a[c][0] = *reinterpret_cast<const f2*>(ar + c * T);
+                a[c][0] = *reinterpret_cast<const pair*>(ar + c * T);
             }
         }
-        float b[Q];
-        const float* br = b_ptr + k * ldb;
+        R b[Q];
+        const R* br = b_ptr + k * ldb;
+        if constexpr (sizeof(R) == 4) {
 #pragma unroll
-        for (int q4 = 0; q4 < Q / 4; ++q4) {
-            const float4 v = *reinterpret_cast<const float4*>(br + 4 * q4);
-            b[4 * q4 + 0] = v.x;
-            b[4 * q4 + 1] = v.y;
-            b[4 * q4 + 2] = v.z;
-            b[4 * q4 + 3] = v.w;
+            for (int q4 = 0; q4 < Q / 4; ++q4) {
+                const float4 v = *reinterpret_cast<const float4*>(br + 4 * q4);
+                b[4 * q4 + 0] = v.x;
+                b[4 * q4 + 1] = v.y;
+                b[4 * q4 + 2] = v.z;
+                b[4 * q4 + 3] = v.w;
+            }
+        } else {
+#pragma unroll
+            for (int q2 = 0; q2 < Q / 2; ++q2) {
+                const double2 v = *reinterpret_cast<const double2*>(br + 2 * q2);
+                b[2 * q2 + 0] = v.x;
+                b[2 * q2 + 1] = v.y;
+            }
         }
 #pragma unroll
         for (int q = 0; q < Q; ++q) {
-            const f2 bb = pack2(b[q], b[q]);
+            const pair bb = pack2(b[q], b[q]);
 #pragma unroll
             for (int c = 0; c < C; ++c)
 #pragma unroll
@@ -378,9 +449,9 @@ __device__ __forceinline__ void gemm_rows(f2 (&acc)[Q][C][P / 2], const float* _
 }
 
 // scalar view of a packed accumulator tile (p is a compile-time constant after unrolling)
-template <int P>
-__device__ __forceinline__ float pick(const f2 (&v)[P / 2], int p) {
-    const float2 t = unpack2(v[p >> 1]);
+template <int P, typename PairT>
+__device__ __forceinline__ auto pick(const PairT (&v)[P / 2], int p) {
+    const auto t = unpack2(v[p >> 1]);
     return (p & 1) ? t.y : t.x;
 }
 

@@ -1,9 +1,12 @@
 // pinnjet_inst.cu -- one translation unit per jet-channel scheme: compiled with -DPJ_N1=.. -DPJ_N2=.. (see build.py).
-// PJ_N1 = PJ_N2 = -1 builds the scheme-independent K2b reduce.
+// PJ_N1 = PJ_N2 = -1 builds the scheme-independent K2b reduce.  PJ_F64=1 builds the double FFMA kernels of the scheme
+// (launch_k1_f64_*, launch_k2_f64_*, occupancy_f64_*) from the same source; the tensor-core kernels are float only.
 #include "pinnjet_k1.cuh"
 #include "pinnjet_k2.cuh"
+#if !PJ_F64
 #include "pinnjet_k1tc3.cuh"
 #include "pinnjet_k2tc2.cuh"
+#endif
 
 #ifndef PJ_WL
 #define PJ_WL 0
@@ -11,6 +14,19 @@
 #define PJ_CAT4(a, b, c, d) a##b##_##c##_##d
 #define PJ_NAME4(prefix, n1, n2, wl) PJ_CAT4(prefix, n1, n2, wl)
 #define PJ_NAME(prefix, n1, n2) PJ_NAME4(prefix, n1, n2, PJ_WL)
+#if PJ_F64
+#define PJ_PREFIX_K1 launch_k1_f64_
+#define PJ_PREFIX_K2 launch_k2_f64_
+#define PJ_PREFIX_OCC occupancy_f64_
+#define PJ_K1_KERNEL k1_forward_kernel_f64
+#define PJ_K2_KERNEL k2_backward_kernel_f64
+#else
+#define PJ_PREFIX_K1 launch_k1_
+#define PJ_PREFIX_K2 launch_k2_
+#define PJ_PREFIX_OCC occupancy_
+#define PJ_K1_KERNEL k1_forward_kernel
+#define PJ_K2_KERNEL k2_backward_kernel
+#endif
 
 namespace pj {
 
@@ -18,9 +34,10 @@ namespace pj {
 
 // K2b: grad_theta[i] += sum over CTAs of partial[cta][i].  Block = 32 parameters x 8 groups of partials (one warp per group:
 // coalesced 128-byte rows, ~17 dependent adds per thread for 132 partials); fixed summation order -> run-to-run reproducible.
-__global__ void __launch_bounds__(RED_PARAMS * RED_GROUPS) k2_reduce_kernel(const float* __restrict__ gpart, int n_parts, long long n_theta,
-                                                                             float* __restrict__ grad) {
-    __shared__ float red[RED_GROUPS][RED_PARAMS];
+template <typename R>
+__global__ void __launch_bounds__(RED_PARAMS * RED_GROUPS) k2_reduce_kernel(const R* __restrict__ gpart, int n_parts, long long n_theta,
+                                                                             R* __restrict__ grad) {
+    __shared__ R red[RED_GROUPS][RED_PARAMS];
     pdl_launch_dependents();
     pdl_wait();                               // the reverse kernel's partials
     const int il = threadIdx.x & (RED_PARAMS - 1), g = threadIdx.x / RED_PARAMS;
@@ -30,16 +47,34 @@ __global__ void __launch_bounds__(RED_PARAMS * RED_GROUPS) k2_reduce_kernel(cons
     if (g == 0 && i < n_theta) grad[i] += red_combine(red, il);
 }
 
+template <typename R>
+static cudaError_t launch_reduce_t(const R* gpart, int n_parts, long long n_theta, R* grad, cudaStream_t s) {
+    return launch_kernel(k2_reduce_kernel<R>, dim3((unsigned)((n_theta + RED_PARAMS - 1) / RED_PARAMS)), dim3(RED_PARAMS * RED_GROUPS), 0, s,
+                         true, gpart, n_parts, n_theta, grad);
+}
 cudaError_t launch_reduce(const float* gpart, int n_parts, long long n_theta, float* grad, cudaStream_t s) {
-    return launch_kernel(k2_reduce_kernel, dim3((unsigned)((n_theta + RED_PARAMS - 1) / RED_PARAMS)), dim3(RED_PARAMS * RED_GROUPS), 0, s, true,
-                         gpart, n_parts, n_theta, grad);
+    return launch_reduce_t(gpart, n_parts, n_theta, grad, s);
+}
+cudaError_t launch_reduce_f64(const double* gpart, int n_parts, long long n_theta, double* grad, cudaStream_t s) {
+    return launch_reduce_t(gpart, n_parts, n_theta, grad, s);
 }
 
 #else
 
-constexpr int kP = ffma_tile_points(1 + PJ_N1 + PJ_N2);
+#if PJ_F64
+typedef K1ArgsF64 K1A;
+typedef K2ArgsF64 K2A;
+constexpr int kEsz = 8;
+// the double instances are tuned for one CTA per SM in both kernels: their accumulators take twice the registers
+constexpr int kMinB1_128 = 1, kMinB2_128 = 1;
+#else
+typedef K1Args K1A;
+typedef K2Args K2A;
+constexpr int kEsz = 4;
 // CTAs per SM the register allocation is tuned for (shared memory may allow fewer): 128-thread CTAs share an SM
 constexpr int kMinB1_128 = 3, kMinB2_128 = 2;
+#endif
+constexpr int kP = ffma_tile_points(1 + PJ_N1 + PJ_N2, kEsz);
 
 // The kernel instance a plan selects and its block size.  `ready`: result of raising the instance's dynamic
 // shared-memory limit, done once per instance.
@@ -54,41 +89,45 @@ static Variant<Args> variant(void (*kern)(Args), int threads) {
     return {kern, threads, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT)};
 }
 
-static Variant<K1Args> k1_variant(const Plan& pl) {
+static Variant<K1A> k1_variant(const Plan& pl) {
+#if !PJ_F64
     if (pl.tc) {
         static const auto v = variant(k1tc3_forward_kernel<PJ_N1, PJ_N2, PJ_WL>, K1T_THREADS);
         return v;
     }
+#endif
     if (pl.ntc1 == 128) {
-        static const auto v = variant(k1_forward_kernel<128, kMinB1_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(128));
+        static const auto v = variant(PJ_K1_KERNEL<128, kMinB1_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(128));
         return v;
     }
     if (pl.Q1 == FFMA_Q_WIDE) {
-        static const auto v = variant(k1_forward_kernel<256, 1, kP, FFMA_Q_WIDE, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(256));
+        static const auto v = variant(PJ_K1_KERNEL<256, 1, kP, FFMA_Q_WIDE, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(256));
         return v;
     }
-    static const auto v = variant(k1_forward_kernel<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(256));
+    static const auto v = variant(PJ_K1_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(256));
     return v;
 }
 
-static Variant<K2Args> k2_variant(const Plan& pl) {
+static Variant<K2A> k2_variant(const Plan& pl) {
+#if !PJ_F64
     if (pl.tc) {
         static const auto v = variant(k2tc2_backward_kernel<PJ_N1, PJ_N2, PJ_WL>, K2T_THREADS);
         return v;
     }
+#endif
     if (pl.n_out_max > K2_OUT_GROUP) {
         if (pl.ntc == 128) {
-            static const auto v = variant(k2_backward_kernel<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, true>, ffma_k2_threads(128));
+            static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, true>, ffma_k2_threads(128));
             return v;
         }
-        static const auto v = variant(k2_backward_kernel<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, true>, ffma_k2_threads(256));
+        static const auto v = variant(PJ_K2_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, true>, ffma_k2_threads(256));
         return v;
     }
     if (pl.ntc == 128) {
-        static const auto v = variant(k2_backward_kernel<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, false>, ffma_k2_threads(128));
+        static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, false>, ffma_k2_threads(128));
         return v;
     }
-    static const auto v = variant(k2_backward_kernel<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, false>, ffma_k2_threads(256));
+    static const auto v = variant(PJ_K2_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, false>, ffma_k2_threads(256));
     return v;
 }
 
@@ -98,23 +137,23 @@ static cudaError_t launch(const Variant<Args>& v, const Args& a, int grid, int s
     return launch_kernel(v.kern, dim3(grid), dim3(v.threads), smem, s, true, a);
 }
 
-cudaError_t PJ_NAME(launch_k1_, PJ_N1, PJ_N2)(const K1Args& a, int grid, int smem, cudaStream_t s) {
+cudaError_t PJ_NAME(PJ_PREFIX_K1, PJ_N1, PJ_N2)(const K1A& a, int grid, int smem, cudaStream_t s) {
     return launch(k1_variant(a.plan), a, grid, smem, s);
 }
 
-cudaError_t PJ_NAME(launch_k2_, PJ_N1, PJ_N2)(const K2Args& a, int grid, int smem, cudaStream_t s) {
+cudaError_t PJ_NAME(PJ_PREFIX_K2, PJ_N1, PJ_N2)(const K2A& a, int grid, int smem, cudaStream_t s) {
     return launch(k2_variant(a.plan), a, grid, smem, s);
 }
 
 // resident CTAs per SM of the K1 (k = 1) or K2 (k = 2) instance the plan selects, with `smem` bytes of dynamic shared memory
-int PJ_NAME(occupancy_, PJ_N1, PJ_N2)(const Plan& pl, int k, int smem) {
+int PJ_NAME(PJ_PREFIX_OCC, PJ_N1, PJ_N2)(const Plan& pl, int k, int smem) {
     int n = 0;
     cudaError_t e;
     if (k == 1) {
-        const Variant<K1Args> v = k1_variant(pl);
+        const Variant<K1A> v = k1_variant(pl);
         e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, v.kern, v.threads, smem);
     } else {
-        const Variant<K2Args> v = k2_variant(pl);
+        const Variant<K2A> v = k2_variant(pl);
         e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, v.kern, v.threads, smem);
     }
     return e == cudaSuccess ? n : -1;

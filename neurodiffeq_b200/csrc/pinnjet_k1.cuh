@@ -18,9 +18,9 @@ namespace pj {
 
 // ---- producer warp: stream the hidden->hidden weight matrices of every tile, in consumption order -------------------
 // forward order: net 0..n-1, Linear l = 1..L-1, row chunks ascending.  backward (K2): Linear l = L-1..1.
-template <bool kForward>
-__device__ __forceinline__ void weight_producer(const PjSpec& sp, const Plan& pl, const float* __restrict__ pack,
-                                                float* ring, uint64_t* full, uint64_t* empty, int my_tiles) {
+template <bool kForward, typename R>
+__device__ __forceinline__ void weight_producer(const PjSpec& sp, const Plan& pl, const R* __restrict__ pack,
+                                                R* ring, uint64_t* full, uint64_t* empty, int my_tiles) {
     const bool resident = kForward ? pl.resident_fwd : pl.resident_bwd;
     const int n_stage = kForward ? pl.n_stage : pl.n_stage_bwd;
     const int tiles = resident ? (my_tiles > 0 ? 1 : 0) : my_tiles;
@@ -32,15 +32,15 @@ __device__ __forceinline__ void weight_producer(const PjSpec& sp, const Plan& pl
                 const int l = kForward ? li : (L - li);
                 const int rows = kForward ? pl.hp[n][l] : pl.hp[n][l + 1];
                 const int cols = kForward ? pl.hp[n][l + 1] : pl.hp[n][l];
-                const float* src = pack + (kForward ? pl.b_wt[n][l] : pl.b_wo[n][l]);
-                const int rpc = CHUNK_FLOATS / cols;
+                const R* src = pack + (kForward ? pl.b_wt[n][l] : pl.b_wo[n][l]);
+                const int rpc = chunk_elems(sizeof(R)) / cols;
                 for (int r0 = 0; r0 < rows; r0 += rpc, ++it) {
                     const int nr = min(rpc, rows - r0);
                     const int stage = it % n_stage;
                     if (it >= n_stage) mbar_wait(&empty[stage], ((it / n_stage) - 1) & 1);
-                    const uint32_t bytes = (uint32_t)(nr * cols) * 4u;
+                    const uint32_t bytes = (uint32_t)(nr * cols) * (uint32_t)sizeof(R);
                     mbar_arrive_expect_tx(&full[stage], bytes);
-                    tma_bulk_g2s(ring + (size_t)stage * CHUNK_FLOATS, src + (size_t)r0 * cols, bytes, &full[stage]);
+                    tma_bulk_g2s(ring + (size_t)stage * chunk_elems(sizeof(R)), src + (size_t)r0 * cols, bytes, &full[stage]);
                 }
             }
         }
@@ -48,16 +48,17 @@ __device__ __forceinline__ void weight_producer(const PjSpec& sp, const Plan& pl
 }
 
 // consumer-side cursor over the same chunk sequence
+template <typename R>
 struct RingCursor {
     int it;          // streaming: global chunk index; resident: chunk index within the tile
     int n_stage;
     bool resident;
     uint64_t *full, *empty;
-    float* ring;
-    __device__ __forceinline__ const float* acquire() {
+    R* ring;
+    __device__ __forceinline__ const R* acquire() {
         const int stage = it % n_stage;
         mbar_wait(&full[stage], resident ? 0u : (uint32_t)((it / n_stage) & 1));
-        return ring + (size_t)stage * CHUNK_FLOATS;
+        return ring + (size_t)stage * chunk_elems(sizeof(R));
     }
     __device__ __forceinline__ void release(int lane) {
         if (!resident) {
@@ -70,17 +71,17 @@ struct RingCursor {
 
 // z-jets of P points of one unit (registers) -> workspace record (train), activation-jet rule, a-jets -> shared memory.
 // Record channel 0 holds tanh(z0) for tanh nets (the reverse pass then needs no transcendental) and z0 for sin nets.
-template <int P, int N1, int N2, int WL>
-__device__ __forceinline__ void finish_unit(float (&zq)[P][1 + N1 + N2], int act_kind, float* __restrict__ act_row, int T,
-                                            float* __restrict__ rec_row, int T2, const float (&wq)[P][WL > 0 ? WL : 1]) {
+template <int P, int N1, int N2, int WL, typename R>
+__device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2], int act_kind, R* __restrict__ act_row, int T,
+                                            R* __restrict__ rec_row, int T2, const R (&wq)[P][WL > 0 ? WL : 1]) {
     constexpr int C = 1 + N1 + N2;
-    auto store = [](float* dst, const float (&v)[P][C], int c) {
+    auto store = [](R* dst, const R (&v)[P][C], int c) {
         if constexpr (P == 4)
-            *reinterpret_cast<float4*>(dst) = make_float4(v[0][c], v[1][c], v[2][c], v[3][c]);
+            store4(dst, v[0][c], v[1][c], v[2][c], v[3][c]);
         else
-            *reinterpret_cast<float2*>(dst) = make_float2(v[0][c], v[1][c]);
+            store2(dst, v[0][c], v[1][c]);
     };
-    float z0s[P];
+    R z0s[P];
 #pragma unroll
     for (int p = 0; p < P; ++p) z0s[p] = zq[p][0];
     if (rec_row) {
@@ -95,16 +96,17 @@ __device__ __forceinline__ void finish_unit(float (&zq)[P][1 + N1 + N2], int act
             for (int p = 0; p < P; ++p) z0s[p] = zq[p][0];
         }
         if constexpr (P == 4)
-            *reinterpret_cast<float4*>(rec_row) = make_float4(z0s[0], z0s[1], z0s[2], z0s[3]);
+            store4(rec_row, z0s[0], z0s[1], z0s[2], z0s[3]);
         else
-            *reinterpret_cast<float2*>(rec_row) = make_float2(z0s[0], z0s[1]);
+            store2(rec_row, z0s[0], z0s[1]);
     }
 #pragma unroll
     for (int c = 0; c < C; ++c) store(act_row + c * T, zq, c);
 }
 
-template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL>
-__global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(const __grid_constant__ K1Args A) {
+template <typename R, int NTC, int P, int Q, int N1, int N2, int WL>
+__device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
+    typedef typename Pair<R>::type pair;
     constexpr int C = 1 + N1 + N2;
     // service warps after the compute warps: 128-thread CTAs (weights always resident: the producer only issues the initial
     // loads) use ONE warp as producer-then-program warp; 256-thread CTAs have a producer warp and a program warp
@@ -113,15 +115,15 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
     extern __shared__ __align__(128) unsigned char smem[];
     const PjSpec& sp = A.spec;
     const Plan& pl = A.plan;
-    float* act = reinterpret_cast<float*>(smem + pl.k1_act);
-    float* ring = reinterpret_cast<float*>(smem + pl.k1_ring);
-    float* small = reinterpret_cast<float*>(smem + pl.k1_small);
-    float* ycache = reinterpret_cast<float*>(smem + pl.k1_ycache);
-    float* slots = reinterpret_cast<float*>(smem + pl.k1_slots);
+    R* act = reinterpret_cast<R*>(smem + pl.k1_act);
+    R* ring = reinterpret_cast<R*>(smem + pl.k1_ring);
+    R* small = reinterpret_cast<R*>(smem + pl.k1_small);
+    R* ycache = reinterpret_cast<R*>(smem + pl.k1_ycache);
+    R* slots = reinterpret_cast<R*>(smem + pl.k1_slots);
     int4* prog_s = reinterpret_cast<int4*>(smem + pl.k1_prog);
     int4* progw_s = reinterpret_cast<int4*>(smem + pl.k1_progw);      // weight program (WL > 0)
-    float* wbuf = reinterpret_cast<float*>(smem + pl.k1_wbuf);       // [n_nets*WL][T] weights of this tile's points
-    float* wslots = reinterpret_cast<float*>(smem + pl.k1_wslots);   // value file of the weight program (compute threads)
+    R* wbuf = reinterpret_cast<R*>(smem + pl.k1_wbuf);       // [n_nets*WL][T] weights of this tile's points
+    R* wslots = reinterpret_cast<R*>(smem + pl.k1_wslots);   // value file of the weight program (compute threads)
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + pl.k1_misc);
     uint64_t* empty = full + MAX_STAGES;
     uint64_t* yfull = empty + MAX_STAGES;    // [2] jet table of a batch complete -> program warp
@@ -162,22 +164,22 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
     if (warp == N_CWARPS + N_SVC - 1) {   // ---------------- program warp: residual program of batch b while the compute warps
         //                                             already work on the tiles of batch b+1 ----------------
         const bool train_pw = A.mode == 1;
-        float my_sumsq = 0.0f;
+        R my_sumsq = 0.0f;
         const int n_batches = (my_tiles + tiles_per_batch - 1) / tiles_per_batch;
         for (int b = 0; b < n_batches; ++b) {
             const int buf = b & 1;
             mbar_wait(&yfull[buf], (uint32_t)((b >> 1) & 1));
-            const float* yb = ycache + (size_t)buf * sp.n_yrows * EB;
+            const R* yb = ycache + (size_t)buf * sp.n_yrows * EB;
             const int first_iter = b * tiles_per_batch;
             const int npts = min(tiles_per_batch, my_tiles - first_iter) * T;
             for (int bp = lane; bp < npts; bp += 32) {
                 const int tl = bp / T, pt = bp - tl * T;
                 const long long btile = (long long)blockIdx.x + (long long)(first_iter + tl) * gridDim.x;
                 const long long gidx = btile * T + pt;
-                float* seed_tile = (train_pw && gidx < ws_points)
+                R* seed_tile = (train_pw && gidx < ws_points)
                                        ? A.seeds + (gidx / T2) * ((long long)sp.n_yrows * T2) + (gidx % T2) : nullptr;
                 if (gidx < A.N) {
-                    ProgIO io{A.coords, gidx, A.N, yb + bp, EB, A.rbar, A.loss_scale, A.u_out, A.r_out, seed_tile, T2};
+                    ProgIOT<R> io{A.coords, gidx, A.N, yb + bp, EB, A.rbar, A.loss_scale, A.u_out, A.r_out, seed_tile, T2};
                     my_sumsq += run_program<32>(prog_s, A.prog_len, slots + lane, io);
                 } else if (seed_tile) {
                     for (int r = 0; r < sp.n_yrows; ++r) seed_tile[r * T2] = 0.0f;   // padded points: zero adjoint
@@ -195,7 +197,7 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
     // -------------------------------------------- compute warps --------------------------------------------------------
     const JobMap jm(tid, T, P, Q);
     const int p0 = jm.p0, u0 = jm.u0;
-    RingCursor cur{0, pl.n_stage, pl.resident_fwd != 0, full, empty, ring};
+    RingCursor<R> cur{0, pl.n_stage, pl.resident_fwd != 0, full, empty, ring};
     const bool train = A.mode == 1;
     int bslot = 0, batch_idx = 0;   // tile slot inside the current batch, batches handed to the program warp so far
     PJ_T_DECL   // slots: 0 setup, 1 layer0, 2 gemm, 3 barrier-after-gemm, 4 epilogue, 5 output layer, 6 program
@@ -206,7 +208,7 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
         const long long base = tile * T;
         if (cur.resident) cur.it = 0;
         if (bslot == 0 && batch_idx >= 2) mbar_wait(&yempty[batch_idx & 1], (uint32_t)(((batch_idx >> 1) - 1) & 1));
-        float* yb = ycache + (size_t)(batch_idx & 1) * sp.n_yrows * EB + bslot * T;
+        R* yb = ycache + (size_t)(batch_idx & 1) * sp.n_yrows * EB + bslot * T;
         // z-jet record of this thread's P points: K2-tile index and column inside it
         if (iter + 1 < my_tiles) {   // pull the next tile's coordinates towards L1 while this tile computes
             const long long nb = (tile + gridDim.x) * T + p0;
@@ -214,11 +216,11 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
                 for (int i = 0; i < sp.n_coords; ++i) asm volatile("prefetch.global.L1 [%0];" ::"l"(A.coords[i] + nb));
         }
         const bool rec = train && (base + p0 < ws_points);
-        float* zj_tile = rec ? A.zj + ((base + p0) / T2) * pl.zj_tile_floats + (p0 % T2) : nullptr;
+        R* zj_tile = rec ? A.zj + ((base + p0) / T2) * pl.zj_tile_floats + (p0 % T2) : nullptr;
         if constexpr (WL > 0) {   // per-point weights of the combined second-order channel (coordinate-only expressions)
             const int NW = sp.n_nets * WL;
             if (tid < T) {
-                ProgIO io{A.coords, min(base + tid, A.N - 1), A.N, nullptr, 0, nullptr, 0.0f, nullptr, nullptr, nullptr, T2};
+                ProgIOT<R> io{A.coords, min(base + tid, A.N - 1), A.N, nullptr, 0, nullptr, 0.0f, nullptr, nullptr, nullptr, T2};
                 io.w_out = wbuf + tid;
                 io.w_stride = T;
                 run_program<NTC>(progw_s, A.prog_w_len, wslots + tid, io);
@@ -236,7 +238,7 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
             const PjNet& net = sp.net[n];
             const int L = net.n_linear - 1;   // hidden layers
             const int act_kind = net.act;
-            float wq[P][WL > 0 ? WL : 1];
+            R wq[P][WL > 0 ? WL : 1];
 #pragma unroll
             for (int p = 0; p < P; ++p)
 #pragma unroll
@@ -246,10 +248,10 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
             {
                 const int hp1 = pl.hp[n][1];
                 if (u0 < hp1) {
-                    const float* wt0 = small + pl.s_wt0[n];
-                    const float* b0 = small + pl.s_b[n][0];
-                    const float* dzt = small + pl.s_dz[n];
-                    float x[PJ_MAX_COORDS][P];
+                    const R* wt0 = small + pl.s_wt0[n];
+                    const R* b0 = small + pl.s_b[n][0];
+                    const R* dzt = small + pl.s_dz[n];
+                    R x[PJ_MAX_COORDS][P];
 #pragma unroll
                     for (int i = 0; i < PJ_MAX_COORDS; ++i)
                         if (i < net.n_in) {
@@ -259,23 +261,23 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
                                 x[i][p] = __ldg(A.coords[net.in_coord[i]] + g);
                             }
                         }
-                    float* zrow = rec ? zj_tile + pl.zj_off[n][1] : nullptr;
+                    R* zrow = rec ? zj_tile + pl.zj_off[n][1] : nullptr;
 #pragma unroll
                     for (int q = 0; q < Q; ++q) {
                         const int u = u0 + q;
-                        float w[PJ_MAX_COORDS];
+                        R w[PJ_MAX_COORDS];
 #pragma unroll
                         for (int i = 0; i < PJ_MAX_COORDS; ++i) w[i] = (i < net.n_in) ? wt0[i * hp1 + u] : 0.0f;
-                        float dz[N1 > 0 ? N1 : 1];
+                        R dz[N1 > 0 ? N1 : 1];
 #pragma unroll
                         for (int f = 0; f < N1; ++f) dz[f] = dzt[f * hp1 + u];
-                        float zq[P][C];
+                        R zq[P][C];
 #pragma unroll
                         for (int p = 0; p < P; ++p) {
-                            float s = b0[u];
+                            R s = b0[u];
 #pragma unroll
                             for (int i = 0; i < PJ_MAX_COORDS; ++i)
-                                if (i < net.n_in) s = fmaf(w[i], x[i][p], s);
+                                if (i < net.n_in) s = fma(w[i], x[i][p], s);
                             zq[p][0] = s;
 #pragma unroll
                             for (int f = 0; f < N1; ++f) zq[p][1 + f] = dz[f];
@@ -293,16 +295,16 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
             for (int l = 1; l < L; ++l) {
                 const int K = pl.hp[n][l], NO = pl.hp[n][l + 1];
                 const bool valid = u0 < NO;
-                f2 acc[Q][C][P / 2];
+                pair acc[Q][C][P / 2];
 #pragma unroll
                 for (int q = 0; q < Q; ++q)
 #pragma unroll
                     for (int c = 0; c < C; ++c)
 #pragma unroll
-                        for (int h = 0; h < P / 2; ++h) acc[q][c][h] = 0ull;
-                const int rpc = CHUNK_FLOATS / NO;
+                        for (int h = 0; h < P / 2; ++h) acc[q][c][h] = pair{};
+                const int rpc = chunk_elems(sizeof(R)) / NO;
                 for (int r0 = 0; r0 < K; r0 += rpc) {
-                    const float* chunk = cur.acquire();
+                    const R* chunk = cur.acquire();
                     if (valid) gemm_rows<P, Q, C>(acc, act + r0 * RS + p0, RS, T, chunk + u0, NO, min(rpc, K - r0));
                     cur.release(lane);
                 }
@@ -310,13 +312,13 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
                 bar_compute<NTC>();   // every read of the previous layer's jets is done -> overwrite in place
                 PJ_T_MARK(3)
                 if (valid) {
-                    const float* bl = small + pl.s_b[n][l];
-                    float* zrow = rec ? zj_tile + pl.zj_off[n][l + 1] : nullptr;
+                    const R* bl = small + pl.s_b[n][l];
+                    R* zrow = rec ? zj_tile + pl.zj_off[n][l + 1] : nullptr;
 #pragma unroll
                     for (int q = 0; q < Q; ++q) {
                         const int u = u0 + q;
-                        const float bias = bl[u];
-                        float zq[P][C];
+                        const R bias = bl[u];
+                        R zq[P][C];
 #pragma unroll
                         for (int c = 0; c < C; ++c)
 #pragma unroll
@@ -331,20 +333,20 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
             // ---------------- last Linear: hidden L -> raw outputs, all channels, into the batch jet table -------------
             {
                 const int hpL = pl.hp[n][L], n_out = net.width[net.n_linear];
-                const float* wl = small + pl.s_wlt[n];
-                const float* bo = small + pl.s_bout[n];
+                const R* wl = small + pl.s_wlt[n];
+                const R* bo = small + pl.s_bout[n];
                 const int rows = n_out * C;
                 for (int e = tid; e < rows * T; e += NT_COMPUTE) {
                     const int pt = e % T, row = e / T, o = row / C, c = row - o * C;
-                    const float* ap = act + c * T + pt;
-                    const float* wp = wl + o;
-                    float s0 = (c == 0) ? bo[o] : 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;   // 4 chains: latency, not order
+                    const R* ap = act + c * T + pt;
+                    const R* wp = wl + o;
+                    R s0 = (c == 0) ? bo[o] : 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;   // 4 chains: latency, not order
 #pragma unroll 2
                     for (int k = 0; k < hpL; k += 4) {   // hpL is a multiple of 32
-                        s0 = fmaf(wp[(k + 0) * n_out], ap[(k + 0) * RS], s0);
-                        s1 = fmaf(wp[(k + 1) * n_out], ap[(k + 1) * RS], s1);
-                        s2 = fmaf(wp[(k + 2) * n_out], ap[(k + 2) * RS], s2);
-                        s3 = fmaf(wp[(k + 3) * n_out], ap[(k + 3) * RS], s3);
+                        s0 = fma(wp[(k + 0) * n_out], ap[(k + 0) * RS], s0);
+                        s1 = fma(wp[(k + 1) * n_out], ap[(k + 1) * RS], s1);
+                        s2 = fma(wp[(k + 2) * n_out], ap[(k + 2) * RS], s2);
+                        s3 = fma(wp[(k + 3) * n_out], ap[(k + 3) * RS], s3);
                     }
                     yb[(net.yrow0 + row) * EB + pt] = (s0 + s1) + (s2 + s3);
                 }
@@ -361,6 +363,16 @@ __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(
         }
     }
     PJ_T_FLUSH(0)
+}
+
+// The float and double kernels: one body (element type R); the float instance keeps its name and argument type.
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL>
+__global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(const __grid_constant__ K1Args A) {
+    k1_forward_body<float, NTC, P, Q, N1, N2, WL>(A);
+}
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL>
+__global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel_f64(const __grid_constant__ K1ArgsF64 A) {
+    k1_forward_body<double, NTC, P, Q, N1, N2, WL>(A);
 }
 
 }  // namespace pj

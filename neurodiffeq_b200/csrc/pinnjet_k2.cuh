@@ -20,41 +20,42 @@ namespace pj {
 constexpr int WJ = 8, WK = 4;   // weight-gradient output tile per thread (8 rows of z_bar x 4 rows of a-jets)
 
 // out[j][k] += sum_r G[j][r] * Z[k][r],  r over the C*T (channel, point) pairs; rows interleaved over lanes so that the
-// float4 loads of 8 consecutive rows (stride RS = C*T+4 floats) hit 32 distinct banks.
-__device__ __forceinline__ void wgrad_tile(f2 (&acc)[WJ][WK], const float* __restrict__ g_base, int j_step,
-                                           const float* __restrict__ z_base, int k_step, int RS, int R) {
+// 16-byte loads of 8 consecutive rows (stride RS = C*T + 16 bytes) hit 32 distinct banks.
+template <typename R>
+__device__ __forceinline__ void wgrad_tile(typename Pair<R>::type (&acc)[WJ][WK], const R* __restrict__ g_base, int j_step,
+                                           const R* __restrict__ z_base, int k_step, int RS, int n_r) {
+    typedef typename Pair<R>::row16 row16;
+    constexpr int STEP = 16 / sizeof(R);
 #pragma unroll 2
-    for (int r = 0; r < R; r += 4) {
-        ulonglong2 gv[WJ], zv[WK];
+    for (int r = 0; r < n_r; r += STEP) {
+        row16 gv[WJ], zv[WK];
 #pragma unroll
-        for (int i = 0; i < WJ; ++i) gv[i] = *reinterpret_cast<const ulonglong2*>(g_base + (size_t)i * j_step * RS + r);
+        for (int i = 0; i < WJ; ++i) gv[i] = *reinterpret_cast<const row16*>(g_base + (size_t)i * j_step * RS + r);
 #pragma unroll
-        for (int i = 0; i < WK; ++i) zv[i] = *reinterpret_cast<const ulonglong2*>(z_base + (size_t)i * k_step * RS + r);
+        for (int i = 0; i < WK; ++i) zv[i] = *reinterpret_cast<const row16*>(z_base + (size_t)i * k_step * RS + r);
 #pragma unroll
         for (int i = 0; i < WJ; ++i)
 #pragma unroll
-            for (int j = 0; j < WK; ++j) {
-                ffma2(acc[i][j], gv[i].x, zv[j].x);
-                ffma2(acc[i][j], gv[i].y, zv[j].y);
-            }
+            for (int j = 0; j < WK; ++j) Pair<R>::fma16(acc[i][j], gv[i], zv[j]);
     }
 }
 
 // WIDE: some net has more than K2_OUT_GROUP outputs (a separate instance: the <= 4-output code stays as it is)
-template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, bool WIDE>
-__global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
+template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, bool WIDE>
+__device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
+    typedef typename Pair<R>::type pair;
     constexpr int C = 1 + N1 + N2;
     constexpr int NT_COMPUTE = NTC, NT_TOTAL = NTC + 32, N_CWARPS = NTC / 32;
     extern __shared__ __align__(128) unsigned char smem[];
     const PjSpec& sp = A.spec;
     const Plan& pl = A.plan;
-    float* G = reinterpret_cast<float*>(smem + pl.k2_g0);    // adjoint of the current layer's z-jets
-    float* G2 = reinterpret_cast<float*>(smem + pl.k2_g1);   // ... of the layer below (being produced)
-    float* Zb = reinterpret_cast<float*>(smem + pl.k2_zb);   // z-jets -> a-jets of the layer below
-    float* ring = reinterpret_cast<float*>(smem + pl.k2_ring);
-    float* small = reinterpret_cast<float*>(smem + pl.k2_small);
-    float* ybar = reinterpret_cast<float*>(smem + pl.k2_ybar);
-    float* sgrad = reinterpret_cast<float*>(smem + pl.k2_sgrad);
+    R* G = reinterpret_cast<R*>(smem + pl.k2_g0);    // adjoint of the current layer's z-jets
+    R* G2 = reinterpret_cast<R*>(smem + pl.k2_g1);   // ... of the layer below (being produced)
+    R* Zb = reinterpret_cast<R*>(smem + pl.k2_zb);   // z-jets -> a-jets of the layer below
+    R* ring = reinterpret_cast<R*>(smem + pl.k2_ring);
+    R* small = reinterpret_cast<R*>(smem + pl.k2_small);
+    R* ybar = reinterpret_cast<R*>(smem + pl.k2_ybar);
+    R* sgrad = reinterpret_cast<R*>(smem + pl.k2_sgrad);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + pl.k2_misc);
     uint64_t* empty = full + MAX_STAGES;
     uint64_t* zfull = empty + MAX_STAGES;
@@ -62,7 +63,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int T = pl.T, RS = pl.RS;
     const int my_tiles = (pl.n_tiles > (int)blockIdx.x) ? (pl.n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-    float* gpart = A.gpart + (size_t)blockIdx.x * sp.n_theta;
+    R* gpart = A.gpart + (size_t)blockIdx.x * sp.n_theta;
 
     if (tid == 0) {
         for (int s = 0; s < MAX_STAGES; ++s) {
@@ -87,8 +88,8 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
     const JobMap jm(tid, T, P, Q);
     const int p0 = jm.p0, u0 = jm.u0;
     // every (point-group block, unit) pair is owned by exactly one lane -> private accumulation, no atomics
-    float* sg = sgrad + (size_t)(warp % ((T / P) >> 3)) * pl.sgrad_floats;
-    RingCursor cur{0, pl.n_stage_bwd, pl.resident_bwd != 0, full, empty, ring};
+    R* sg = sgrad + (size_t)(warp % ((T / P) >> 3)) * pl.sgrad_floats;
+    RingCursor<R> cur{0, pl.n_stage_bwd, pl.resident_bwd != 0, full, empty, ring};
     uint32_t zphase = 0;
     // lane mapping of the weight-gradient GEMM: 8 k-lanes x 4 j-lanes per warp
     const int kl = lane & 7, jl = lane >> 3;
@@ -99,8 +100,8 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
         const long long tile = (long long)blockIdx.x + (long long)iter * gridDim.x;
         const long long base = tile * T;
         if (cur.resident) cur.it = 0;
-        const float* zj_tile = A.zj + tile * pl.zj_tile_floats;
-        const float* seed_tile = A.seeds + tile * ((long long)sp.n_yrows * T);
+        const R* zj_tile = A.zj + tile * pl.zj_tile_floats;
+        const R* seed_tile = A.seeds + tile * ((long long)sp.n_yrows * T);
 
         for (int n = 0; n < sp.n_nets; ++n) {
             const PjNet& net = sp.net[n];
@@ -108,7 +109,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
             const int act_kind = net.act;
             const int n_out = net.width[net.n_linear];
             const int hpL = pl.hp[n][L];
-            float wq[P][WL > 0 ? WL : 1];   // weights of the combined second-order channel at this thread's points
+            R wq[P][WL > 0 ? WL : 1];   // weights of the combined second-order channel at this thread's points
 #pragma unroll
             for (int p = 0; p < P; ++p)
 #pragma unroll
@@ -118,7 +119,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
             // (0) seeds of this net + bulk load of the last hidden layer's z-jets
             if (tid == 0) {
                 fence_proxy_async();
-                const uint32_t bytes = (uint32_t)(hpL * RS) * 4u;
+                const uint32_t bytes = (uint32_t)(hpL * RS) * (uint32_t)sizeof(R);
                 mbar_arrive_expect_tx(zfull, bytes);
                 tma_bulk_g2s(Zb, zj_tile + pl.zj_off[n][L], bytes, zfull);
             }
@@ -133,22 +134,22 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
             // a-jets replace the z-jets in Zb (each (unit, point) element belongs to one thread), then one pass per group
             // of K2_OUT_GROUP outputs reduces W_out rows two at a time.
             {
-                const float* wlo = small + pl.s_wlo[n];
+                const R* wlo = small + pl.s_wlo[n];
                 if constexpr (!WIDE) if (u0 < hpL) {
                     static_assert(Q == 4, "the gradient reductions below assume 4 units per thread");
                     static_assert(K2_OUT_GROUP == PJ_MAX_NETS, "the first group's reduction below is written for 4 outputs");
-                    float gbq[Q], gwq[K2_OUT_GROUP][Q];   // per-thread partials: bias of hidden L, W_out rows of one group
+                    R gbq[Q], gwq[K2_OUT_GROUP][Q];   // per-thread partials: bias of hidden L, W_out rows of one group
 #pragma unroll
                     for (int q = 0; q < Q; ++q) {
                         const int u = u0 + q;
-                        float gw[K2_OUT_GROUP];
+                        R gw[K2_OUT_GROUP];
 #pragma unroll
                         for (int o = 0; o < K2_OUT_GROUP; ++o) gw[o] = 0.0f;
-                        float gb = 0.0f;
+                        R gb = 0.0f;
 #pragma unroll
                         for (int p = 0; p < P; ++p) {
                             const int pt = p0 + p;
-                            float z[C], ab[C], a[C], zb[C];
+                            R z[C], ab[C], a[C], zb[C];
 #pragma unroll
                             for (int c = 0; c < C; ++c) {
                                 z[c] = Zb[u * RS + c * T + pt];
@@ -157,16 +158,16 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
 #pragma unroll
                             for (int o = 0; o < K2_OUT_GROUP; ++o)
                                 if (o < n_out) {
-                                    const float w = wlo[o * hpL + u];
+                                    const R w = wlo[o * hpL + u];
 #pragma unroll
-                                    for (int c = 0; c < C; ++c) ab[c] = fmaf(w, ybar[(o * C + c) * T + pt], ab[c]);
+                                    for (int c = 0; c < C; ++c) ab[c] = fma(w, ybar[(o * C + c) * T + pt], ab[c]);
                                 }
                             act_backward<N1, N2, WL>(act_kind, z, ab, a, zb, wq[p]);
 #pragma unroll
                             for (int o = 0; o < K2_OUT_GROUP; ++o)
                                 if (o < n_out) {
 #pragma unroll
-                                    for (int c = 0; c < C; ++c) gw[o] = fmaf(ybar[(o * C + c) * T + pt], a[c], gw[o]);
+                                    for (int c = 0; c < C; ++c) gw[o] = fma(ybar[(o * C + c) * T + pt], a[c], gw[o]);
                                 }
                             gb += zb[0];
 #pragma unroll
@@ -178,42 +179,42 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                     }
                     const int pl8 = jm.pg_lane, i4 = pl8 & 3;
                     {   // reduce over the point lanes: [bias(4) | W_out row 0 (4)], then W_out rows 1.. two at a time
-                        const float v0[8] = {gbq[0], gbq[1], gbq[2], gbq[3], gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3]};
-                        const float t0 = pg_reduce_scatter8(v0, pl8);
+                        const R v0[8] = {gbq[0], gbq[1], gbq[2], gbq[3], gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3]};
+                        const R t0 = pg_reduce_scatter8(v0, pl8);
                         if (pl8 < 4) sg[pl.g_b[n][L - 1] + u0 + i4] += t0; else sg[pl.g_wl[n] + u0 + i4] += t0;
                         if (n_out > 1) {
-                            const float v1[8] = {gwq[1][0], gwq[1][1], gwq[1][2], gwq[1][3],
+                            const R v1[8] = {gwq[1][0], gwq[1][1], gwq[1][2], gwq[1][3],
                                                  gwq[2][0], gwq[2][1], gwq[2][2], gwq[2][3]};
-                            const float t1 = pg_reduce_scatter8(v1, pl8);
+                            const R t1 = pg_reduce_scatter8(v1, pl8);
                             if (pl8 < 4) sg[pl.g_wl[n] + hpL + u0 + i4] += t1;
                             else if (n_out > 2) sg[pl.g_wl[n] + 2 * hpL + u0 + i4] += t1;
                         }
                         if (n_out > 3) {
-                            const float v2[4] = {gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
-                            const float t2 = pg_reduce_scatter4(v2, pl8);
+                            const R v2[4] = {gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
+                            const R t2 = pg_reduce_scatter4(v2, pl8);
                             if (!(pl8 & 1)) sg[pl.g_wl[n] + 3 * hpL + u0 + (pl8 >> 1)] += t2;
                         }
                     }
                 }
                 if constexpr (WIDE) if (u0 < hpL) {
-                    float gbq[Q];
+                    R gbq[Q];
 #pragma unroll
                     for (int q = 0; q < Q; ++q) {
                         const int u = u0 + q;
-                        float gb = 0.0f;
+                        R gb = 0.0f;
 #pragma unroll
                         for (int p = 0; p < P; ++p) {
                             const int pt = p0 + p;
-                            float z[C], ab[C], a[C], zb[C];
+                            R z[C], ab[C], a[C], zb[C];
 #pragma unroll
                             for (int c = 0; c < C; ++c) {
                                 z[c] = Zb[u * RS + c * T + pt];
                                 ab[c] = 0.0f;
                             }
                             for (int o = 0; o < n_out; ++o) {
-                                const float w = wlo[o * hpL + u];
+                                const R w = wlo[o * hpL + u];
 #pragma unroll
-                                for (int c = 0; c < C; ++c) ab[c] = fmaf(w, ybar[(o * C + c) * T + pt], ab[c]);
+                                for (int c = 0; c < C; ++c) ab[c] = fma(w, ybar[(o * C + c) * T + pt], ab[c]);
                             }
                             act_backward<N1, N2, WL>(act_kind, z, ab, a, zb, wq[p]);
                             gb += zb[0];
@@ -226,47 +227,47 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                         gbq[q] = gb;
                     }
                     const int pl8 = jm.pg_lane, i4 = pl8 & 3;
-                    const float tb = pg_reduce_scatter4(gbq, pl8);
+                    const R tb = pg_reduce_scatter4(gbq, pl8);
                     if (!(pl8 & 1)) sg[pl.g_b[n][L - 1] + u0 + (pl8 >> 1)] += tb;
                     for (int o0 = 0; o0 < n_out; o0 += K2_OUT_GROUP) {
-                        float gwq[K2_OUT_GROUP][Q];
+                        R gwq[K2_OUT_GROUP][Q];
 #pragma unroll
                         for (int q = 0; q < Q; ++q) {
                             const int u = u0 + q;
-                            float gw[K2_OUT_GROUP];
+                            R gw[K2_OUT_GROUP];
 #pragma unroll
                             for (int o = 0; o < K2_OUT_GROUP; ++o) gw[o] = 0.0f;
 #pragma unroll
                             for (int p = 0; p < P; ++p) {
                                 const int pt = p0 + p;
-                                float a[C];
+                                R a[C];
 #pragma unroll
                                 for (int c = 0; c < C; ++c) a[c] = Zb[u * RS + c * T + pt];
 #pragma unroll
                                 for (int o = 0; o < K2_OUT_GROUP; ++o)
                                     if (o0 + o < n_out) {
 #pragma unroll
-                                        for (int c = 0; c < C; ++c) gw[o] = fmaf(ybar[((o0 + o) * C + c) * T + pt], a[c], gw[o]);
+                                        for (int c = 0; c < C; ++c) gw[o] = fma(ybar[((o0 + o) * C + c) * T + pt], a[c], gw[o]);
                                     }
                             }
 #pragma unroll
                             for (int o = 0; o < K2_OUT_GROUP; ++o) gwq[o][q] = gw[o];
                         }
                         const int row = o0 + (pl8 >> 2);   // reduced value pl8: unit u0 + (pl8 & 3) of row o0 (+1 for pl8 >= 4)
-                        const float v1[8] = {gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3],
+                        const R v1[8] = {gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3],
                                              gwq[1][0], gwq[1][1], gwq[1][2], gwq[1][3]};
-                        const float t1 = pg_reduce_scatter8(v1, pl8);
+                        const R t1 = pg_reduce_scatter8(v1, pl8);
                         if (row < n_out) sg[pl.g_wl[n] + row * hpL + u0 + i4] += t1;
                         if (o0 + 2 < n_out) {
-                            const float v2[8] = {gwq[2][0], gwq[2][1], gwq[2][2], gwq[2][3],
+                            const R v2[8] = {gwq[2][0], gwq[2][1], gwq[2][2], gwq[2][3],
                                                  gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
-                            const float t2 = pg_reduce_scatter8(v2, pl8);
+                            const R t2 = pg_reduce_scatter8(v2, pl8);
                             if (row + 2 < n_out) sg[pl.g_wl[n] + (row + 2) * hpL + u0 + i4] += t2;
                         }
                     }
                 }
                 if (tid < n_out) {   // b_out gradient: sum over points of the value-channel seed
-                    float s = 0.0f;
+                    R s = 0.0f;
                     for (int pt = 0; pt < T; ++pt) s += ybar[(tid * C) * T + pt];
                     sgrad[pl.g_bout[n] + tid] += s;
                 }
@@ -280,22 +281,22 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                 const int HJ = pl.hp[n][h], HK = pl.hp[n][h - 1];
                 if (tid == 0) {   // z-jets of hidden h-1 (Zb is free: every reader passed the barrier above)
                     fence_proxy_async();
-                    const uint32_t bytes = (uint32_t)(HK * RS) * 4u;
+                    const uint32_t bytes = (uint32_t)(HK * RS) * (uint32_t)sizeof(R);
                     mbar_arrive_expect_tx(zfull, bytes);
                     tma_bulk_g2s(Zb, zj_tile + pl.zj_off[n][h - 1], bytes, zfull);
                 }
                 // (2a) a_bar_{h-1} = W_l^T z_bar_h
                 const bool valid = u0 < HK;
-                f2 acc[Q][C][P / 2];
+                pair acc[Q][C][P / 2];
 #pragma unroll
                 for (int q = 0; q < Q; ++q)
 #pragma unroll
                     for (int c = 0; c < C; ++c)
 #pragma unroll
-                        for (int hh = 0; hh < P / 2; ++hh) acc[q][c][hh] = 0ull;
-                const int rpc = CHUNK_FLOATS / HK;
+                        for (int hh = 0; hh < P / 2; ++hh) acc[q][c][hh] = pair{};
+                const int rpc = chunk_elems(sizeof(R)) / HK;
                 for (int r0 = 0; r0 < HJ; r0 += rpc) {
-                    const float* chunk = cur.acquire();
+                    const R* chunk = cur.acquire();
                     if (valid) gemm_rows<P, Q, C>(acc, G + r0 * RS + p0, RS, T, chunk + u0, HK, min(rpc, HJ - r0));
                     cur.release(lane);
                 }
@@ -305,15 +306,15 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                 PJ_T_MARK(4)
                 // (2b) reverse activation of hidden h-1: Zb z-jets -> a-jets (in place), G2 <- z_bar_{h-1}
                 if (valid) {
-                    float gbq[Q];
+                    R gbq[Q];
 #pragma unroll
                     for (int q = 0; q < Q; ++q) {
                         const int u = u0 + q;
-                        float gb = 0.0f;
-                        float av[P][C], zv[P][C];
+                        R gb = 0.0f;
+                        R av[P][C], zv[P][C];
 #pragma unroll
                         for (int p = 0; p < P; ++p) {
-                            float z[C], ab[C];
+                            R z[C], ab[C];
 #pragma unroll
                             for (int c = 0; c < C; ++c) {
                                 z[c] = Zb[u * RS + c * T + p0 + p];
@@ -325,18 +326,16 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
 #pragma unroll
                         for (int c = 0; c < C; ++c) {
                             if constexpr (P == 4) {
-                                *reinterpret_cast<float4*>(Zb + u * RS + c * T + p0) =
-                                    make_float4(av[0][c], av[1][c], av[2][c], av[3][c]);
-                                *reinterpret_cast<float4*>(G2 + u * RS + c * T + p0) =
-                                    make_float4(zv[0][c], zv[1][c], zv[2][c], zv[3][c]);
+                                store4(Zb + u * RS + c * T + p0, av[0][c], av[1][c], av[2][c], av[3][c]);
+                                store4(G2 + u * RS + c * T + p0, zv[0][c], zv[1][c], zv[2][c], zv[3][c]);
                             } else {
-                                *reinterpret_cast<float2*>(Zb + u * RS + c * T + p0) = make_float2(av[0][c], av[1][c]);
-                                *reinterpret_cast<float2*>(G2 + u * RS + c * T + p0) = make_float2(zv[0][c], zv[1][c]);
+                                store2(Zb + u * RS + c * T + p0, av[0][c], av[1][c]);
+                                store2(G2 + u * RS + c * T + p0, zv[0][c], zv[1][c]);
                             }
                         }
                         gbq[q] = gb;
                     }
-                    const float tb = pg_reduce_scatter4(gbq, jm.pg_lane);
+                    const R tb = pg_reduce_scatter4(gbq, jm.pg_lane);
                     if (!(jm.pg_lane & 1)) sg[pl.g_b[n][h - 2] + u0 + (jm.pg_lane >> 1)] += tb;
                 }
                 bar_compute<NTC>();
@@ -345,14 +344,14 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                 {
                     const int width_j = net.width[h], width_k = net.width[h - 1];   // unpadded
                     const int n_kb = HK / 32, n_jb = HJ / 32;   // warp tile = 32 rows j x 32 rows k
-                    float* gw = gpart + net.w_off[l];
+                    R* gw = gpart + net.w_off[l];
                     for (int wt = warp; wt < n_kb * n_jb; wt += N_CWARPS) {
                         const int jb = (wt / n_kb) * 32, kb = (wt % n_kb) * 32;
-                        f2 wacc[WJ][WK];
+                        pair wacc[WJ][WK];
 #pragma unroll
                         for (int i = 0; i < WJ; ++i)
 #pragma unroll
-                            for (int jj = 0; jj < WK; ++jj) wacc[i][jj] = 0ull;
+                            for (int jj = 0; jj < WK; ++jj) wacc[i][jj] = pair{};
                         wgrad_tile(wacc, G + (size_t)(jb + jl) * RS, 4, Zb + (size_t)(kb + kl) * RS, 8, RS, C * T);
                         // every output element is owned by one thread of this CTA, so the fire-and-forget reduction
                         // (RED.ADD, no return value to wait for) into the CTA's private partial is race-free and ordered
@@ -363,7 +362,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                             for (int jj = 0; jj < WK; ++jj) {
                                 const int k = kb + kl + 8 * jj;
                                 if (j < width_j && k < width_k) {
-                                    const float2 v = unpack2(wacc[i][jj]);
+                                    const auto v = unpack2(wacc[i][jj]);
                                     atomicAdd(&gw[(size_t)j * width_k + k], v.x + v.y);
                                 }
                             }
@@ -372,7 +371,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
                 }
                 bar_compute<NTC>();
                 PJ_T_MARK(6)
-                float* t = G;
+                R* t = G;
                 G = G2;
                 G2 = t;
             }
@@ -381,7 +380,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
             {
                 const int hp1 = pl.hp[n][1];
                 if (u0 < hp1) {
-                    float x[PJ_MAX_COORDS][P];
+                    R x[PJ_MAX_COORDS][P];
 #pragma unroll
                     for (int i = 0; i < PJ_MAX_COORDS; ++i)
                         if (i < net.n_in) {
@@ -394,8 +393,8 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
 #pragma unroll
                     for (int q = 0; q < Q; ++q) {
                         const int u = u0 + q;
-                        float s0[P];
-                        float sf[N1 > 0 ? N1 : 1];
+                        R s0[P];
+                        R sf[N1 > 0 ? N1 : 1];
 #pragma unroll
                         for (int f = 0; f < N1; ++f) sf[f] = 0.0f;
 #pragma unroll
@@ -404,25 +403,25 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
 #pragma unroll
                             for (int f = 0; f < N1; ++f) sf[f] += G[u * RS + (1 + f) * T + p0 + p];
                         }
-                        float sv[PJ_MAX_COORDS];
+                        R sv[PJ_MAX_COORDS];
 #pragma unroll
                         for (int i = 0; i < PJ_MAX_COORDS; ++i) {
-                            float s = 0.0f;
+                            R s = 0.0f;
                             if (i < net.n_in) {
 #pragma unroll
-                                for (int p = 0; p < P; ++p) s = fmaf(s0[p], x[i][p], s);
+                                for (int p = 0; p < P; ++p) s = fma(s0[p], x[i][p], s);
 #pragma unroll
-                                for (int f = 0; f < N1; ++f) s = fmaf(sf[f], sp.dir[f][net.in_coord[i]], s);
+                                for (int f = 0; f < N1; ++f) s = fma(sf[f], R(sp.dir[f][net.in_coord[i]]), s);
                             }
                             sv[i] = s;
                         }
                         if (net.n_in <= 4) {
-                            const float v4[4] = {sv[0], sv[1], sv[2], sv[3]};
-                            const float t = pg_reduce_scatter4(v4, jm.pg_lane);
+                            const R v4[4] = {sv[0], sv[1], sv[2], sv[3]};
+                            const R t = pg_reduce_scatter4(v4, jm.pg_lane);
                             const int i = jm.pg_lane >> 1;
                             if (!(jm.pg_lane & 1) && i < net.n_in) sg[pl.g_w0[n] + u * net.n_in + i] += t;
                         } else {
-                            const float t = pg_reduce_scatter8(sv, jm.pg_lane);
+                            const R t = pg_reduce_scatter8(sv, jm.pg_lane);
                             if (jm.pg_lane < net.n_in) sg[pl.g_w0[n] + u * net.n_in + jm.pg_lane] += t;
                         }
                     }
@@ -441,7 +440,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
         const int L = net.n_linear - 1;
         const int h1 = net.width[1], hL = net.width[L], hpL = pl.hp[n][L], n_out = net.width[net.n_linear];
         auto sgsum = [&](int idx) {
-            float v = 0.0f;
+            R v = 0.0f;
             for (int c = 0; c < pl.sgrad_copies; ++c) v += sgrad[(size_t)c * pl.sgrad_floats + idx];
             return v;
         };
@@ -454,6 +453,16 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
         }
         for (int e = tid; e < n_out; e += NT_COMPUTE) gpart[net.b_off[L] + e] += sgsum(pl.g_bout[n] + e);
     }
+}
+
+// The float and double kernels: one body (element type R); the float instance keeps its name and argument type.
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, bool WIDE>
+__global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
+    k2_backward_body<float, NTC, P, Q, N1, N2, WL, WIDE>(A);
+}
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, bool WIDE>
+__global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel_f64(const __grid_constant__ K2ArgsF64 A) {
+    k2_backward_body<double, NTC, P, Q, N1, N2, WL, WIDE>(A);
 }
 
 }  // namespace pj

@@ -26,35 +26,35 @@ static int hidden_linears(const PjSpec& sp) {   // hidden->hidden Linears of all
 
 // ---- shared-memory images ----
 
-int k1_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, int prog_len, int prog_w_len, SmemImage* regions) {
+int k1_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, int prog_len, int prog_w_len, SmemImage* regions, int esz) {
     SmemImage img;
     // act | ring | small | ycache | slots | misc | wbuf | wslots | prog | progw
-    img.place(pl.k1_act, "act", pl.hmax * pl.RS1 * 4);
-    img.place(pl.k1_ring, "ring", n_stage * CHUNK_FLOATS * 4);
-    img.place(pl.k1_small, "small", round_up(pl.small_floats * 4, 128));
-    img.place(pl.k1_ycache, "ycache", 2 * sp.n_yrows * pl.epi_batch * 4);
-    img.place(pl.k1_slots, "slots", sp.n_slots * 32 * 4);
+    img.place(pl.k1_act, "act", pl.hmax * pl.RS1 * esz);
+    img.place(pl.k1_ring, "ring", n_stage * CHUNK_BYTES);
+    img.place(pl.k1_small, "small", round_up(pl.small_floats * esz, 128));
+    img.place(pl.k1_ycache, "ycache", 2 * sp.n_yrows * pl.epi_batch * esz);
+    img.place(pl.k1_slots, "slots", sp.n_slots * 32 * esz);
     img.place(pl.k1_misc, "misc", 256);
-    img.place(pl.k1_wbuf, "wbuf", sp.n_nets * sp.wl * pl.T1 * 4);
-    img.place(pl.k1_wslots, "wslots", sp.wl > 0 ? sp.n_slots * pl.ntc1 * 4 : 0);
+    img.place(pl.k1_wbuf, "wbuf", sp.n_nets * sp.wl * pl.T1 * esz);
+    img.place(pl.k1_wslots, "wslots", sp.wl > 0 ? sp.n_slots * pl.ntc1 * esz : 0);
     img.place(pl.k1_prog, "prog", prog_len * 16);
     img.place(pl.k1_progw, "progw", prog_w_len * 16);
     if (regions) *regions = img;
     return img.bytes;
 }
 
-int k2_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, SmemImage* regions) {
+int k2_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, SmemImage* regions, int esz) {
     SmemImage img;
     // G | G2 | Zb | ring | small | ybar | sgrad | misc
-    const int jet_bytes = pl.hmax * pl.RS * 4;
+    const int jet_bytes = pl.hmax * pl.RS * esz;
     img.place(pl.k2_g0, "g0", jet_bytes);
     img.place(pl.k2_g1, "g1", jet_bytes);
     img.place(pl.k2_zb, "zb", jet_bytes);
-    img.place(pl.k2_ring, "ring", n_stage * CHUNK_FLOATS * 4);
-    img.place(pl.k2_small, "small", round_up(pl.small_floats * 4, 128));
+    img.place(pl.k2_ring, "ring", n_stage * CHUNK_BYTES);
+    img.place(pl.k2_small, "small", round_up(pl.small_floats * esz, 128));
     const int ybar_rows = pl.n_out_max > K2_OUT_GROUP ? pl.n_out_max : K2_OUT_GROUP;
-    img.place(pl.k2_ybar, "ybar", round_up(ybar_rows * pl.C * pl.T * 4, 128));
-    img.place(pl.k2_sgrad, "sgrad", round_up(pl.sgrad_floats * pl.sgrad_copies * 4, 128));
+    img.place(pl.k2_ybar, "ybar", round_up(ybar_rows * pl.C * pl.T * esz, 128));
+    img.place(pl.k2_sgrad, "sgrad", round_up(pl.sgrad_floats * pl.sgrad_copies * esz, 128));
     img.place(pl.k2_misc, "misc", 256);
     if (regions) *regions = img;
     return img.bytes;
@@ -96,14 +96,15 @@ int k2_tc_layout(const PjSpec& sp, Plan& pl, SmemImage* regions) {
 }
 
 // Weight-ring depth: keep all chunks resident if that still allows `target_occ` CTAs per SM; otherwise stream with as many
-// stages as fit (>= 2), giving up one CTA per SM at a time.  Returns -1 if nothing fits.
-static int pick_stages(int fixed_bytes, int chunks, int target_occ, bool resident_only = false) {
-    if (chunks == 0) return fixed_bytes <= SMEM_LIMIT ? 1 : -1;
+// stages as fit (>= 2), giving up one CTA per SM at a time.  Returns -1 if nothing fits.  Without hidden->hidden weights
+// the float plans keep one (unused) stage; the double plans, whose jet buffers are twice as large, none.
+static int pick_stages(int fixed_bytes, int chunks, int target_occ, bool resident_only, int esz) {
+    if (chunks == 0) return fixed_bytes <= SMEM_LIMIT ? (esz == 4 ? 1 : 0) : -1;
     const int per_sm = SMEM_PER_SM - 1024;   // minus the reserve of the system
     for (int occ = target_occ; occ >= 1; --occ) {
         int budget = per_sm / occ - 1024;
         if (budget > SMEM_LIMIT) budget = SMEM_LIMIT;
-        int ns = (budget - fixed_bytes) / (CHUNK_FLOATS * 4);
+        int ns = (budget - fixed_bytes) / CHUNK_BYTES;
         if (ns > MAX_STAGES) ns = MAX_STAGES;
         if (ns > chunks) ns = chunks;
         if (ns >= chunks || (ns >= 2 && !resident_only)) return ns;
@@ -126,11 +127,11 @@ struct Err {
 }  // namespace
 
 // K1 tile of the FFMA kernel for `ntc1` compute threads (a multiple of the K2 tile T); false if the shape is unsupported
-static bool set_k1_tile(Plan& pl, int ntc1, long long N) {
+static bool set_k1_tile(Plan& pl, int ntc1, long long N, int esz) {
     pl.ntc1 = ntc1;
     pl.T1 = pl.ntc1 * pl.P1 * pl.Q1 / pl.hmax;
     if ((pl.T1 / pl.P1) % 8 != 0 || pl.T1 % pl.T != 0) return false;
-    pl.RS1 = pl.C * pl.T1 + ROW_PAD;
+    pl.RS1 = pl.C * pl.T1 + row_pad(esz);
     pl.epi_batch = pl.T1 > 32 ? pl.T1 : 32;   // whole tiles; the program warp walks it 32 points at a time
     pl.n_tiles1 = (int)((N + pl.T1 - 1) / pl.T1);
     return true;
@@ -138,7 +139,7 @@ static bool set_k1_tile(Plan& pl, int ntc1, long long N) {
 
 // Everything the kernels need to agree on, for K2 CTAs of `ntc` compute threads.
 static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_len, int ntc_req, const PlanDevice& dev,
-                        Plan& pl, int* occ_min, const Err& fail) {
+                        Plan& pl, int* occ_min, const Err& fail, int esz) {
     memset(&pl, 0, sizeof(pl));
     if (sp.abi_version != PJ_ABI_VERSION) return fail(-1, "PjSpec.abi_version %d != %d", sp.abi_version, PJ_ABI_VERSION);
     if (sp.n_nets < 1 || sp.n_nets > PJ_MAX_NETS) return fail(-1, "n_nets=%d out of range", sp.n_nets);
@@ -149,7 +150,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     if (sp.wl < 0 || sp.wl > sp.n1 || (sp.wl > 0 && sp.n2 != 1)) return fail(-1, "inconsistent wl=%d (n1=%d, n2=%d)", sp.wl, sp.n1, sp.n2);
     const int C = 1 + sp.n1 + sp.n2;
     pl.C = C;
-    pl.P = ffma_tile_points(C);
+    pl.P = ffma_tile_points(C, esz);
     pl.Q = FFMA_Q;
     int hmax = 32, yrows = 0;
     for (int n = 0; n < sp.n_nets; ++n) {
@@ -180,13 +181,13 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     if (ntc_req == 128 && hmax > 64) return fail(-3, "internal: 128-thread CTAs need hidden width <= 64");
     pl.T = pl.ntc * pl.P * pl.Q / hmax;
     if ((pl.T / pl.P) % 8 != 0 || pl.T > pl.ntc) return fail(-3, "internal: tile %d unsupported", pl.T);
-    pl.RS = C * pl.T + ROW_PAD;
+    pl.RS = C * pl.T + row_pad(esz);
     pl.n_tiles = (int)((N + pl.T - 1) / pl.T);
     // K1: 8 units per thread (half the shared-memory wavefronts per FFMA of the 4-unit tile); its tile is a multiple of T
     pl.P1 = pl.P;
     pl.Q1 = hmax > 64 ? FFMA_Q_WIDE : FFMA_Q;   // wide nets are GEMM-bound (fewer smem wavefronts); narrow ones want more CTAs per SM
-    const bool k1_ok = set_k1_tile(pl, hmax <= 64 ? 128 : 256, N) ||
-                       (pl.T1 < pl.T && set_k1_tile(pl, 256, N));   // K2 fell back to one 256-thread CTA per SM: give K1 the same tile
+    const bool k1_ok = set_k1_tile(pl, hmax <= 64 ? 128 : 256, N, esz) ||
+                       (pl.T1 < pl.T && set_k1_tile(pl, 256, N, esz));   // K2 fell back to one 256-thread CTA per SM: give K1 the same tile
     if (!k1_ok) return fail(-3, "internal: forward tile %d unsupported (backward tile %d)", pl.T1, pl.T);
 
     // ---- packed parameters ----
@@ -210,11 +211,14 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
             const int hi = pl.hp[n][l], ho = pl.hp[n][l + 1];
             pl.b_wt[n][l] = big; big += (long long)hi * ho;
             pl.b_wo[n][l] = big; big += (long long)hi * ho;
-            pl.b_wimg[n][l] = big; big += 3 * TC_WIMG / 4;   // three bf16 images [64 x 64] (used by the tensor-core path)
-            pl.chunks_fwd += (hi + CHUNK_FLOATS / ho - 1) / (CHUNK_FLOATS / ho);
-            pl.chunks_bwd += (ho + CHUNK_FLOATS / hi - 1) / (CHUNK_FLOATS / hi);
+            pl.b_wimg[n][l] = big;
+            if (esz == 4) big += 3 * TC_WIMG / 4;   // three bf16 images [64 x 64] (used by the tensor-core path)
+            const int ce = chunk_elems(esz);
+            pl.chunks_fwd += (hi + ce / ho - 1) / (ce / ho);
+            pl.chunks_bwd += (ho + ce / hi - 1) / (ce / hi);
         }
-        pl.b_woutimg[n] = big; big += 3 * TC_WOUT / 4;   // three bf16 images [16 x 64] of the output Linear (tensor-core path)
+        pl.b_woutimg[n] = big;
+        if (esz == 4) big += 3 * TC_WOUT / 4;   // three bf16 images [16 x 64] of the output Linear (tensor-core path)
     }
     pl.pack_floats = big;
 
@@ -236,7 +240,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     // most 4 outputs per net (one 16-byte row of the output Linear), the weight images of both kernels resident in shared
     // memory.  The decision may not depend on the program length (only
     // pj_forward* know it): the programs get a fixed reserve.
-    bool tc = dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4;
+    bool tc = esz == 4 && dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4;
     for (int n = 0; tc && n < sp.n_nets; ++n)
         for (int h = 1; h < sp.net[n].n_linear; ++h) tc = tc && pl.hp[n][h] == TC_H;
     if (tc) {   // both kernels tile like the forward kernel; seeds / weights / records are shared as is
@@ -275,21 +279,21 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
         // CTA per SM with a streamed ring -- its tile stays a multiple of the record tile T.
         int ns = -1;
         for (int attempt = 0; attempt < 2 && ns < 0; ++attempt) {
-            if (attempt == 1 && (pl.ntc1 == 256 || !set_k1_tile(pl, 256, N))) break;
+            if (attempt == 1 && (pl.ntc1 == 256 || !set_k1_tile(pl, 256, N, esz))) break;
             // 128-thread forward CTAs share one service warp between weight loading and the residual program -> resident only
-            const int fixed = k1_ffma_layout(sp, pl, 0, prog_len, prog_w_len);
-            ns = pick_stages(fixed, pl.chunks_fwd, pl.ntc1 == 128 ? 3 : 1, pl.ntc1 == 128);
+            const int fixed = k1_ffma_layout(sp, pl, 0, prog_len, prog_w_len, nullptr, esz);
+            ns = pick_stages(fixed, pl.chunks_fwd, pl.ntc1 == 128 ? 3 : 1, pl.ntc1 == 128, esz);
         }
         if (ns < 0) return fail(-2, "forward kernel does not fit in shared memory");
         pl.n_stage = ns;
         pl.resident_fwd = ns >= pl.chunks_fwd;
-        pl.k1_bytes = k1_ffma_layout(sp, pl, ns, prog_len, prog_w_len);
+        pl.k1_bytes = k1_ffma_layout(sp, pl, ns, prog_len, prog_w_len, nullptr, esz);
 
-        const int ns2 = pick_stages(k2_ffma_layout(sp, pl, 0), pl.chunks_bwd, pl.ntc == 128 ? 2 : 1);
+        const int ns2 = pick_stages(k2_ffma_layout(sp, pl, 0, nullptr, esz), pl.chunks_bwd, pl.ntc == 128 ? 2 : 1, false, esz);
         if (ns2 < 0) return fail(-2, "backward kernel does not fit in shared memory");
         pl.n_stage_bwd = ns2;
         pl.resident_bwd = ns2 >= pl.chunks_bwd ? 1 : 0;
-        pl.k2_bytes = k2_ffma_layout(sp, pl, ns2);
+        pl.k2_bytes = k2_ffma_layout(sp, pl, ns2, nullptr, esz);
     }
 
     // ---- persistent grids: resident CTAs per SM x SMs, capped by the number of tiles ----
@@ -301,7 +305,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
         pl.grid = pl.n_tiles1 < dev.sms * o1 ? pl.n_tiles1 : dev.sms * o1;
         pl.grid_bwd = pl.n_tiles < dev.sms * o2 ? pl.n_tiles : dev.sms * o2;
         const int parts_per_cta = pl.tc ? K1T_NPW : 1;   // K1-TC: one partial per program warp
-        if (pl.grid * parts_per_cta > MAX_LOSS_PARTS) pl.grid = MAX_LOSS_PARTS / parts_per_cta;
+        if (pl.grid * parts_per_cta > max_loss_parts(esz)) pl.grid = max_loss_parts(esz) / parts_per_cta;
         pl.n_loss_parts = parts_per_cta * pl.grid;
         *occ_min = pl.tc ? 2 : o2;   // (the tensor-core plan does not depend on the CTA shape: accept it at once)
     }
@@ -312,10 +316,11 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     pl.zj_tile_floats = zt;
     pl.ws_loss = 0;
     pl.ws_zj = LOSS_PART_BYTES;
-    pl.ws_seed = round_up_ll(pl.ws_zj + (pl.tc ? 0ll : 4ll * zt * pl.n_tiles), 256);
-    pl.ws_gpart = round_up_ll(pl.ws_seed + 4ll * sp.n_yrows * pl.T * pl.n_tiles, 256);
-    pl.ws_wts = round_up_ll(pl.ws_gpart + 4ll * sp.n_theta * pl.grid_bwd, 256);
-    pl.ws_tcrec = round_up_ll(pl.ws_wts + 4ll * sp.n_nets * sp.wl * pl.T * pl.n_tiles, 256);
+    const long long e = esz;
+    pl.ws_seed = round_up_ll(pl.ws_zj + (pl.tc ? 0ll : e * zt * pl.n_tiles), 256);
+    pl.ws_gpart = round_up_ll(pl.ws_seed + e * sp.n_yrows * pl.T * pl.n_tiles, 256);
+    pl.ws_wts = round_up_ll(pl.ws_gpart + e * sp.n_theta * pl.grid_bwd, 256);
+    pl.ws_tcrec = round_up_ll(pl.ws_wts + e * sp.n_nets * sp.wl * pl.T * pl.n_tiles, 256);
     pl.ws_bytes = round_up_ll(pl.ws_tcrec + (pl.tc ? 4ll * pl.tc_rec_tile_floats * pl.n_tiles1 : 0ll), 256);
     return 0;
 }
@@ -323,17 +328,27 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
 // Narrow networks (hidden width <= 64) run 128-thread CTAs when at least two of them fit on an SM in BOTH kernels (their
 // GEMM / activation / program phases then overlap); otherwise one 256-thread CTA per SM.
 int make_plan(const PjSpec& sp, long long N, int prog_len, int prog_w_len, const PlanDevice& dev, Plan& pl, char* err,
-              int err_len) {
+              int err_len, int esz) {
     const Err fail{err, err_len};
+    if (esz != 4 && esz != 8) return fail(-1, "element size %d (4 or 8)", esz);
     int occ = 0, hmax = 0;
     for (int n = 0; n < sp.n_nets && n < PJ_MAX_NETS; ++n)
         for (int h = 1; h < sp.net[n].n_linear && h <= PJ_MAX_LINEAR; ++h)
             if (sp.net[n].width[h] > hmax) hmax = sp.net[n].width[h];
+    Plan narrow;
+    int rc128 = -1;
     if (hmax <= 64) {
-        const int rc = plan_for_ntc(sp, N, prog_len, prog_w_len, 128, dev, pl, &occ, fail);
-        if (rc == 0 && occ >= 2) return 0;
+        rc128 = plan_for_ntc(sp, N, prog_len, prog_w_len, 128, dev, pl, &occ, fail, esz);
+        if (rc128 == 0 && occ >= 2) return 0;
+        narrow = pl;
     }
-    return plan_for_ntc(sp, N, prog_len, prog_w_len, 256, dev, pl, &occ, fail);
+    const int rc = plan_for_ntc(sp, N, prog_len, prog_w_len, 256, dev, pl, &occ, fail, esz);
+    // double jet buffers may not fit a 256-thread tile at all: then one 128-thread CTA per SM is the plan
+    if (rc != 0 && rc128 == 0 && esz == 8) {
+        pl = narrow;
+        return 0;
+    }
+    return rc;
 }
 
 }  // namespace pj

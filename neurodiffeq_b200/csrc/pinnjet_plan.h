@@ -11,11 +11,19 @@ constexpr int SMEM_LIMIT = 232448;       // opt-in maximum of dynamic shared mem
 constexpr int SMEM_PER_SM = 233472;      // shared memory per SM on sm_90 (228 KB)
 
 // ---- FFMA kernels (pinnjet_k1.cuh, pinnjet_k2.cuh) ----
-constexpr int CHUNK_FLOATS = 4096;       // weight chunk = 16 KB
+// Element size `esz`: 4 for the float kernels, 8 for the double ones (the same source, compiled with PJ_F64=1).  Tile
+// shapes, row strides and packed offsets are counted in elements, shared-memory and workspace offsets in bytes.
+constexpr int CHUNK_BYTES = 16384;       // weight chunk
+constexpr int CHUNK_FLOATS = CHUNK_BYTES / 4;
+constexpr int chunk_elems(int esz) { return CHUNK_BYTES / esz; }
 constexpr int MAX_STAGES = 8;
 constexpr int ROW_PAD = 4;               // jet rows are C*T + 4 floats: conflict-free row-strided float4 loads
+// Jet-row padding: 16 bytes (4 floats, 2 doubles), so that the 16-byte row-strided loads of 8 consecutive rows hit 32
+// distinct banks and every row starts 16-byte aligned (bulk TMA).
+constexpr int row_pad(int esz) { return 16 / esz; }
 // Thread tile: P points x Q units.  K2 and narrow-network K1 CTAs use Q = FFMA_Q; K1 of 128-wide networks FFMA_Q_WIDE.
-constexpr int ffma_tile_points(int C) { return C <= 2 ? 4 : 2; }
+// Double accumulators take two registers each: the double kernels use 2-point tiles throughout.
+constexpr int ffma_tile_points(int C, int esz = 4) { return C <= 2 && esz == 4 ? 4 : 2; }
 constexpr int FFMA_Q = 4, FFMA_Q_WIDE = 8;
 // K2 reduces the output-Linear gradient in groups of this many outputs (pinnjet_k2.cuh)
 constexpr int K2_OUT_GROUP = 4;
@@ -53,6 +61,8 @@ constexpr int LOSS_PART_BYTES = 4096;
 constexpr int LOSS_TICKET_WORD = 639;    // counter of the in-kernel loss finalisation (zero between launches)
 constexpr int LOSS_DBG_WORD = 640;       // start of the diagnostics area (written by PJ_TIMING builds only)
 constexpr int MAX_LOSS_PARTS = LOSS_TICKET_WORD;   // partials occupy words [0, n_loss_parts)
+// partials of `esz` bytes that fit below the ticket (639 floats, 319 doubles): the planner caps the forward grid there
+constexpr int max_loss_parts(int esz) { return LOSS_TICKET_WORD * 4 / esz; }
 
 // Everything derived from (spec, N): identical on host and device.
 struct Plan {
@@ -114,9 +124,10 @@ struct SmemImage {
 
 // The layout of each kernel: the only place that assigns its shared-memory offsets.  Each reads the tile fields of `pl`,
 // writes its offset fields and returns the image size (and the regions, if asked).  `n_stage`: weight-ring stages (0
-// gives the size of everything else); program lengths in instructions.
-int k1_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, int prog_len, int prog_w_len, SmemImage* regions = nullptr);
-int k2_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, SmemImage* regions = nullptr);
+// gives the size of everything else); program lengths in instructions; `esz`: element size of the kernel (4 or 8).
+int k1_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, int prog_len, int prog_w_len, SmemImage* regions = nullptr,
+                   int esz = 4);
+int k2_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, SmemImage* regions = nullptr, int esz = 4);
 int k1_tc_layout(const PjSpec& sp, Plan& pl, int prog_len, int prog_w_len, SmemImage* regions = nullptr);
 int k2_tc_layout(const PjSpec& sp, Plan& pl, SmemImage* regions = nullptr);
 
@@ -131,7 +142,9 @@ struct PlanDevice {
 
 // 0 or a negative code with a message in err[0, err_len): -1 invalid spec / arguments, -2 the kernels cannot take the
 // problem, -3 internal inconsistency, -4 the device query failed.  prog_len / prog_w_len move only the K1 image.
+// esz = 8 plans the double kernels: always FFMA (whatever dev.tc_level says), every buffer of 8-byte elements, at most
+// max_loss_parts(8) forward CTAs.  dev.occupancy must then query the double instances.
 int make_plan(const PjSpec& sp, long long N, int prog_len, int prog_w_len, const PlanDevice& dev, Plan& pl, char* err,
-              int err_len);
+              int err_len, int esz = 4);
 
 }  // namespace pj

@@ -24,7 +24,7 @@ class EagerProblem:
     is_eager = True
 
     def __init__(self, nets, conditions, diff_eqs, n_coords, coords_for_condition=None, device=None, aux_outputs=None,
-                 enforce=None, reason=""):
+                 enforce=None, reason="", dtype=None):
         if device is None:
             if not torch.cuda.is_available():
                 raise RuntimeError("the PINN engine needs a CUDA device (H100, sm_90a); none is visible")
@@ -34,7 +34,10 @@ class EagerProblem:
         self.nets, self.conditions, self.diff_eqs = list(nets), list(conditions), diff_eqs
         self.n_coords = n_coords
         self._cfc, self._aux, self._enforce = coords_for_condition, aux_outputs, enforce
-        self.dtype = torch.float32 if self.device.type == "cuda" else torch.get_default_dtype()
+        if dtype is not None:   # float64: the reference's precision, on CUDA as well
+            self.dtype = dtype
+        else:
+            self.dtype = torch.float32 if self.device.type == "cuda" else torch.get_default_dtype()
         self._adopt_parameters()
         self.kernel_launches = 0          # none of ours: the counter stays 0 on this path
         self.jit_reason = "autograd path"
@@ -206,12 +209,13 @@ _WARNED = set()
 
 
 def build_problem(fused_cls, nets, conditions, diff_eqs, n_coords, coords_for_condition=None, device=None, aux_outputs=None,
-                  enforce=None):
+                  enforce=None, **dtype):
     """``fused_cls(...)``, or -- when the tracer / planner refuses the problem -- an :class:`EagerProblem` with one warning per
-    distinct reason.  Errors that are not refusals (no CUDA device, missing library, inconsistent shapes) propagate."""
+    distinct reason.  Errors that are not refusals (no CUDA device, missing library, inconsistent shapes) propagate.
+    ``dtype=...``, when given, reaches both (``torch.float64``: the double kernels, or the autograd path in float64)."""
     try:
         return fused_cls(nets, conditions, diff_eqs, n_coords, coords_for_condition=coords_for_condition, device=device,
-                         aux_outputs=aux_outputs, enforce=enforce)
+                         aux_outputs=aux_outputs, enforce=enforce, **dtype)
     except (NotImplementedError, TypeError) as exc:
         reason = f"{type(exc).__name__}: {exc}"
     if reason not in _WARNED:
@@ -219,4 +223,4 @@ def build_problem(fused_cls, nets, conditions, diff_eqs, n_coords, coords_for_co
         warnings.warn("the fused engine cannot express this problem (" + reason + "); falling back to the autograd path "
                       "(neurodiffeq_b200.eager.EagerProblem: torch.autograd on the device, reference speed)", RuntimeWarning)
     return EagerProblem(nets, conditions, diff_eqs, n_coords, coords_for_condition=coords_for_condition, device=device,
-                        aux_outputs=aux_outputs, enforce=enforce, reason=reason)
+                        aux_outputs=aux_outputs, enforce=enforce, reason=reason, **dtype)

@@ -84,8 +84,17 @@ def load_library():
                                           ctypes.POINTER(ctypes.c_uint64), i32, i32, vp]
     lib.pj_backward_allreduce_bytes.argtypes = [i64, i32]
     lib.pj_backward_allreduce_bytes.restype = i64
+    # float64 twins: same arguments with double buffers (and a double loss_scale)
+    lib.pj_sizes_f64.argtypes = lib.pj_sizes.argtypes
+    lib.pj_plan_info_f64.argtypes = lib.pj_plan_info.argtypes
+    lib.pj_pack_f64.argtypes = lib.pj_pack.argtypes
+    lib.pj_pack_zero_f64.argtypes = lib.pj_pack_zero.argtypes
+    lib.pj_forward_f64.argtypes = lib.pj_forward.argtypes
+    lib.pj_forward_train_f64.argtypes = [ctypes.c_double if t is f32 else t for t in lib.pj_forward_train.argtypes]
+    lib.pj_backward_f64.argtypes = lib.pj_backward.argtypes
     for fn in (lib.pj_sizes, lib.pj_pack, lib.pj_forward, lib.pj_forward_train, lib.pj_backward, lib.pj_forward_jit,
-               lib.pj_forward_train_jit, lib.pj_backward_allreduce):
+               lib.pj_forward_train_jit, lib.pj_backward_allreduce, lib.pj_sizes_f64, lib.pj_plan_info_f64, lib.pj_pack_f64,
+               lib.pj_pack_zero_f64, lib.pj_forward_f64, lib.pj_forward_train_f64, lib.pj_backward_f64):
         fn.restype = ctypes.c_int
     if lib.pj_abi_version() != 2:
         raise RuntimeError("libpinnjet.so ABI version mismatch")
@@ -96,9 +105,11 @@ def load_library():
 EXPORTED_SYMBOLS = ("pj_abi_version", "pj_last_error", "pj_sizes", "pj_plan_info", "pj_pack", "pj_forward", "pj_forward_train",
                     "pj_backward", "pj_allreduce_bytes", "pj_allreduce_oneshot", "pj_sample", "pj_adam_step", "pj_forward_jit",
                     "pj_forward_train_jit", "pj_backward_allreduce_bytes", "pj_backward_allreduce", "pj_pack_zero")
+F64_SYMBOLS = ("pj_sizes_f64", "pj_plan_info_f64", "pj_pack_f64", "pj_pack_zero_f64", "pj_forward_f64", "pj_forward_train_f64",
+               "pj_backward_f64")
 
 
-def planner_refusal(lib, spec, device, n_points=1024):
+def planner_refusal(lib, spec, device, n_points=1024, f64=False):
     """Text of the planner's refusal if the kernels cannot take this problem at all (return code -2 of ``pj_sizes``: hidden
     width > PJ_MAX_WIDTH, more than PJ_MAX_NETS output units, jet table too tall, a kernel that does not fit in shared
     memory, ...), else ``None``.  ``FusedProblem.__init__`` turns it into ``NotImplementedError`` so that the solvers'
@@ -106,7 +117,7 @@ def planner_refusal(lib, spec, device, n_points=1024):
     import contextlib
     ctx = torch.cuda.device(device) if torch.device(device).type == "cuda" else contextlib.nullcontext()
     with ctx:
-        rc = lib.pj_sizes(ctypes.byref(spec), n_points, ctypes.byref(PjSizes()))
+        rc = (lib.pj_sizes_f64 if f64 else lib.pj_sizes)(ctypes.byref(spec), n_points, ctypes.byref(PjSizes()))
     if rc == -2:
         return lib.pj_last_error().decode()
     return None
@@ -136,8 +147,8 @@ class _PinnedStage:
     phase with a single sync per phase)."""
     DEPTH = 2
 
-    def __init__(self, n_cols, n, device):
-        self.bufs = [[torch.empty(n, dtype=torch.float32).pin_memory() for _ in range(n_cols)] for _ in range(self.DEPTH)]
+    def __init__(self, n_cols, n, device, dtype=torch.float32):
+        self.bufs = [[torch.empty(n, dtype=dtype).pin_memory() for _ in range(n_cols)] for _ in range(self.DEPTH)]
         self.done = [[None] * n_cols for _ in range(self.DEPTH)]
         self.turn = [0] * n_cols
         self.device = device
@@ -157,12 +168,29 @@ class _PinnedStage:
         ev.record(torch.cuda.current_stream(self.device))
 
 
+def check_dtype(dtype):
+    """``None`` / ``torch.float32`` (the default) or ``torch.float64``; anything else raises ``ValueError``."""
+    if dtype is None or dtype == torch.float32:
+        return torch.float32
+    if dtype == torch.float64:
+        return torch.float64
+    raise ValueError(f"dtype must be torch.float32 or torch.float64, not {dtype}")
+
+
 class FusedProblem:
-    """Device state for one (nets, conditions, diff_eqs): spec, programs, flat parameter/gradient storage, workspace."""
+    """Device state for one (nets, conditions, diff_eqs): spec, programs, flat parameter/gradient storage, workspace.
+
+    ``dtype=torch.float64`` runs the problem on the double kernels (the ``_f64`` entry points): parameters, gradients,
+    coordinates, outputs and the loss are float64, the networks are converted to float64."""
+
+    dtype, f64, esz = torch.float32, False, 4   # set per instance by __init__
 
     def __init__(self, nets, conditions, diff_eqs, n_coords, coords_for_condition=None, device=None, aux_outputs=None,
-                 enforce=None):
+                 enforce=None, dtype=None):
         self.lib = load_library()
+        self.dtype = check_dtype(dtype)
+        self.f64 = self.dtype == torch.float64
+        self.esz = 8 if self.f64 else 4
         if device is None:
             if not torch.cuda.is_available():
                 raise RuntimeError("the fused PINN engine needs a CUDA device (H100, sm_90a); none is visible")
@@ -181,7 +209,7 @@ class FusedProblem:
         self._const_coord_cache = {}
         self._adopt_parameters()
         self._build_spec()
-        why = planner_refusal(self.lib, self.spec, self.device)
+        why = planner_refusal(self.lib, self.spec, self.device, f64=self.f64)
         if why is not None:
             raise NotImplementedError("the kernels' planner refuses this problem: " + why)
         dev = self.device
@@ -209,19 +237,26 @@ class FusedProblem:
         if os.environ.get("PINNJET_JIT") == "1":
             self.enable_jit()
 
-    # ---- parameters: one flat fp32 buffer, nn.Parameters become views (torch layout preserved) ----------------------
+    def _fn(self, name):
+        """entry point ``name`` of the library, or its float64 twin for a float64 problem"""
+        return getattr(self.lib, name + "_f64" if self.f64 else name)
+
+    def _program(self, program):
+        return program.to_f64() if self.f64 else program
+
+    # ---- parameters: one flat buffer of the problem's dtype, nn.Parameters become views (torch layout preserved) -------
     def _adopt_parameters(self):
         params, seen = [], set()
         for nd in self.tp.nets:   # a module evaluated at two coordinate lists (boundary instance) owns ONE set of weights
-            nd.module.to(device=self.device, dtype=torch.float32)
+            nd.module.to(device=self.device, dtype=self.dtype)
             for p in nd.parameters():
                 if id(p) not in seen:
                     seen.add(id(p))
                     params.append(p)
         n_theta = sum(p.numel() for p in params)
-        self.theta = torch.empty(n_theta, dtype=torch.float32, device=self.device)
+        self.theta = torch.empty(n_theta, dtype=self.dtype, device=self.device)
         # one buffer [grad_theta | sum r^2] so that a multi-GPU step needs a single all-reduce (SURVEY.md §8e)
-        self.gradbuf = torch.zeros(n_theta + 1, dtype=torch.float32, device=self.device)
+        self.gradbuf = torch.zeros(n_theta + 1, dtype=self.dtype, device=self.device)
         self.grad = self.gradbuf[:n_theta]
         self.sumsq = self.gradbuf[n_theta:n_theta + 1]
         self.offsets = []
@@ -241,9 +276,9 @@ class FusedProblem:
     def parameters_linked(self):
         """True while every nn.Parameter still aliases the flat buffers (``net.to()`` / re-assignment break it)."""
         for p, off in zip(self.params, self.offsets):
-            if p.data_ptr() != self.theta.data_ptr() + 4 * off:
+            if p.data_ptr() != self.theta.data_ptr() + self.esz * off or p.dtype != self.dtype:
                 return False
-            if p.grad is None or p.grad.data_ptr() != self.grad.data_ptr() + 4 * off:
+            if p.grad is None or p.grad.data_ptr() != self.grad.data_ptr() + self.esz * off:
                 return False
         return True
 
@@ -251,12 +286,12 @@ class FusedProblem:
         with torch.no_grad():
             for p, off in zip(self.params, self.offsets):
                 n = p.numel()
-                if p.data_ptr() != self.theta.data_ptr() + 4 * off:
-                    self.theta[off:off + n].copy_(p.detach().to(self.device, torch.float32).reshape(-1))
+                if p.data_ptr() != self.theta.data_ptr() + self.esz * off or p.dtype != self.dtype:
+                    self.theta[off:off + n].copy_(p.detach().to(self.device, self.dtype).reshape(-1))
                     p.data = self.theta[off:off + n].view(p.shape)
-                if p.grad is None or p.grad.data_ptr() != self.grad.data_ptr() + 4 * off:
+                if p.grad is None or p.grad.data_ptr() != self.grad.data_ptr() + self.esz * off:
                     if p.grad is not None:
-                        self.grad[off:off + n].copy_(p.grad.detach().to(self.device, torch.float32).reshape(-1))
+                        self.grad[off:off + n].copy_(p.grad.detach().to(self.device, self.dtype).reshape(-1))
                     else:
                         self.grad[off:off + n].zero_()
                     p.grad = self.grad[off:off + n].view(p.shape)
@@ -276,8 +311,8 @@ class FusedProblem:
             for i in range(tp.n_coords):
                 sp.dir[f][i] = float(dirs[f, i])
         sp.n_funcs, sp.n_eq, sp.n_yrows = tp.n_funcs, tp.n_eq, tp.n_yrows
-        sp.n_slots = max(tp.prog_eval.n_slots, tp.prog_train.n_slots, tp.prog_train_ext.n_slots,
-                         tp.prog_w.n_slots if tp.wl else 1)
+        sp.n_slots = max(self._program(p).n_slots for p in (tp.prog_eval, tp.prog_train, tp.prog_train_ext) +
+                         ((tp.prog_w,) if tp.wl else ()))
         sp.n_theta = self.n_theta
         for n, nd in enumerate(tp.nets):
             net = sp.net[n]
@@ -309,15 +344,18 @@ class FusedProblem:
                 for i in range(n_in):
                     self._theta_index[("skip", id(nd.module), o, i)] = base + o * n_in + i
             rows = torch.tensor([tp.yrow0[k] + o * tp.n_channels for o in range(nd.n_out)], device=dev)
-            dirs = torch.as_tensor(tp.direction_matrix()[:, list(nd.in_coord)], dtype=torch.float32, device=dev)
+            dirs = torch.as_tensor(tp.direction_matrix()[:, list(nd.in_coord)], dtype=self.dtype, device=dev)
             self._skips.append((k, base, rows, dirs))
 
     def _upload(self, program):
-        """device copy of a lowered program; remembers which immediates must follow the parameters (Program.patch)"""
+        """device copy of a lowered program (the double lowering for a float64 problem); remembers which immediates must
+        follow the parameters (Program.patch): word a of (op, dst, a, b), or words a and b (low, high) of a double"""
+        program = self._program(program)
         dev_prog = torch.from_numpy(program.code.copy()).to(self.device)
         if program.patch:
             pcs = sorted(program.patch)
-            pos = torch.tensor([pc * 4 + 2 for pc in pcs], dtype=torch.int64, device=self.device)   # (op, dst, IMM, -)
+            words = (2, 3) if self.f64 else (2,)
+            pos = torch.tensor([pc * 4 + w for pc in pcs for w in words], dtype=torch.int64, device=self.device)
             idx = torch.tensor([self._theta_index[program.patch[pc]] for pc in pcs], dtype=torch.int64, device=self.device)
             self._patch_sets.append((dev_prog, pos, idx))
             dev_prog.view(-1)[pos] = self.theta[idx].view(torch.int32)
@@ -336,7 +374,7 @@ class FusedProblem:
             info = self._plan_cache[n] = self.plan_info(n)
         tp = self.tp
         T, nt, n1 = info["T"], info["n_tiles"], tp.scheme.n1
-        raw = self.workspace[info["ws_seed"]: info["ws_seed"] + 4 * tp.n_yrows * T * nt].view(torch.float32)
+        raw = self.workspace[info["ws_seed"]: info["ws_seed"] + self.esz * tp.n_yrows * T * nt].view(self.dtype)
         seeds = raw.view(nt, tp.n_yrows, T).permute(1, 0, 2).reshape(tp.n_yrows, nt * T)[:, :n]      # [n_yrows, N]
         for k, base, rows, dirs in self._skips:
             nd = tp.nets[k]
@@ -351,8 +389,8 @@ class FusedProblem:
         """Prepare for losses that depend on the functions u as well as on the residuals (``ubar`` in
         :meth:`residual_grad`): upload that train program and make the value file large enough for it."""
         if getattr(self, "_prog_train_ext_u", None) is None:
-            p = self.tp.prog_train_ext_u
-            self._prog_train_ext_u = self._upload(p)
+            p = self._program(self.tp.prog_train_ext_u)
+            self._prog_train_ext_u = self._upload(self.tp.prog_train_ext_u)
             if p.n_slots > self.spec.n_slots:
                 self.spec.n_slots = p.n_slots
                 self._sizes_cache.clear()
@@ -371,14 +409,14 @@ class FusedProblem:
         if n_points not in self._sizes_cache:
             out = PjSizes()
             with torch.cuda.device(self.device):
-                _check(self.lib.pj_sizes(ctypes.byref(self.spec), n_points, ctypes.byref(out)), "pj_sizes")
+                _check(self._fn("pj_sizes")(ctypes.byref(self.spec), n_points, ctypes.byref(out)), "pj_sizes")
             self._sizes_cache[n_points] = out
         return self._sizes_cache[n_points]
 
     def _ensure_buffers(self, n_points, train):
         sz = self.sizes(n_points)
         if self.pack_buf is None:
-            self.pack_buf = torch.zeros(sz.pack_bytes // 4, dtype=torch.float32, device=self.device)
+            self.pack_buf = torch.zeros(sz.pack_bytes // self.esz, dtype=self.dtype, device=self.device)
         need = sz.workspace_bytes if train else 4096
         if self.workspace is None or self.workspace.numel() < need:
             self.workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
@@ -396,8 +434,8 @@ class FusedProblem:
         arr = (ctypes.c_void_p * self.tp.n_coords)()
         keep = []
         for i, c in enumerate(coords):
-            if c.device != self.device or c.dtype != torch.float32 or not c.is_contiguous() or c.numel() != n_points:
-                c = c.detach().to(self.device, torch.float32).reshape(-1).contiguous()
+            if c.device != self.device or c.dtype != self.dtype or not c.is_contiguous() or c.numel() != n_points:
+                c = c.detach().to(self.device, self.dtype).reshape(-1).contiguous()
                 if c.numel() != n_points:
                     raise ValueError("all coordinate vectors must have the same number of points")
             keep.append(c)
@@ -405,7 +443,7 @@ class FusedProblem:
         if self.tp.const_coords:   # constant coordinates (network evaluated at a boundary): filled arrays, cached per size
             consts = self._const_coord_cache.get(n_points)
             if consts is None:
-                consts = [torch.full((n_points,), v, dtype=torch.float32, device=self.device) for v in self.tp.const_coords]
+                consts = [torch.full((n_points,), v, dtype=self.dtype, device=self.device) for v in self.tp.const_coords]
                 self._const_coord_cache[n_points] = consts
             for k, c in enumerate(consts):
                 arr[self.n_coords + k] = c.data_ptr()
@@ -413,7 +451,7 @@ class FusedProblem:
         return arr, keep
 
     def _prog_w_args(self):
-        return (self.prog_w.data_ptr(), len(self.tp.prog_w)) if self.tp.wl else (None, 0)
+        return (self.prog_w.data_ptr(), self.prog_w.shape[0]) if self.tp.wl else (None, 0)
 
     # ---- kernels ------------------------------------------------------------------------------------------------------
     def pack(self, zero_gradbuf=False):
@@ -422,10 +460,10 @@ class FusedProblem:
         accumulator of the step, without a fill launch)."""
         self._ensure_buffers(1, False)
         if zero_gradbuf:
-            _check(self.lib.pj_pack_zero(ctypes.byref(self.spec), self.theta.data_ptr(), self.pack_buf.data_ptr(),
+            _check(self._fn("pj_pack_zero")(ctypes.byref(self.spec), self.theta.data_ptr(), self.pack_buf.data_ptr(),
                                          self.gradbuf.data_ptr(), self.gradbuf.numel(), self._stream()), "pj_pack_zero")
         else:
-            _check(self.lib.pj_pack(ctypes.byref(self.spec), self.theta.data_ptr(), self.pack_buf.data_ptr(),
+            _check(self._fn("pj_pack")(ctypes.byref(self.spec), self.theta.data_ptr(), self.pack_buf.data_ptr(),
                                     self._stream()), "pj_pack")
         if self._patch_sets:
             self._apply_patches()
@@ -439,17 +477,17 @@ class FusedProblem:
         if repack:
             self.pack()
         ptrs, keep = self._coord_ptrs(coords, n)
-        u = torch.empty((self.n_funcs, n), dtype=torch.float32, device=self.device) if want_u else None
-        r = torch.empty((self.n_eq, n), dtype=torch.float32, device=self.device) if want_residual else None
+        u = torch.empty((self.n_funcs, n), dtype=self.dtype, device=self.device) if want_u else None
+        r = torch.empty((self.n_eq, n), dtype=self.dtype, device=self.device) if want_residual else None
         if want_sumsq:
             self.sumsq.zero_()
-        args = (ctypes.byref(self.spec), self.prog_eval.data_ptr(), len(self.tp.prog_eval), *self._prog_w_args(), ptrs, n,
+        args = (ctypes.byref(self.spec), self.prog_eval.data_ptr(), self.prog_eval.shape[0], *self._prog_w_args(), ptrs, n,
                 self.pack_buf.data_ptr(), u.data_ptr() if want_u else None, r.data_ptr() if want_residual else None,
                 self.sumsq.data_ptr() if want_sumsq else None, self.workspace.data_ptr(), self.workspace.numel(), self._stream())
         if self._jit_usable(n):
             _check(self.lib.pj_forward_jit(self._jit.function, *args), "pj_forward_jit")
         else:
-            _check(self.lib.pj_forward(*args), "pj_forward")
+            _check(self._fn("pj_forward")(*args), "pj_forward")
         self.kernel_launches += 1          # the loss finalisation happens inside the forward kernel
         return u, r, (self.sumsq if want_sumsq else None)
 
@@ -474,23 +512,24 @@ class FusedProblem:
         ptrs, keep = self._coord_ptrs(coords, n)
         n_glob = n if n_global is None else n_global
         scale = 2.0 / (float(n_glob) * self.n_eq)
-        r = torch.empty((self.n_eq, n), dtype=torch.float32, device=self.device) if want_residual else None
+        r = torch.empty((self.n_eq, n), dtype=self.dtype, device=self.device) if want_residual else None
         if sumsq_out is None:
             sumsq_out = self.sumsq
             sumsq_out.zero_()
         if ubar is not None and rbar is None:
             raise ValueError("ubar (dL/du) needs rbar (dL/dr) as well")
         prog = self.prog_train if rbar is None else self.prog_train_ext
-        prog_len = len(self.tp.prog_train if rbar is None else self.tp.prog_train_ext)
+        prog_len = prog.shape[0]
         if rbar is not None:
-            rbar = rbar.detach().to(self.device, torch.float32).contiguous()
+            rbar = rbar.detach().to(self.device, self.dtype).contiguous()
             if tuple(rbar.shape) != (self.n_eq, n):
                 raise ValueError(f"rbar must have shape ({self.n_eq}, {n})")
         if ubar is not None:   # the external cotangent buffer becomes [dL/dr | dL/du]
-            ubar = ubar.detach().to(self.device, torch.float32).contiguous()
+            ubar = ubar.detach().to(self.device, self.dtype).contiguous()
             if tuple(ubar.shape) != (self.n_funcs, n):
                 raise ValueError(f"ubar must have shape ({self.n_funcs}, {n})")
-            prog, prog_len = self.enable_function_adjoints(), len(self.tp.prog_train_ext_u)
+            prog = self.enable_function_adjoints()
+            prog_len = prog.shape[0]
             rbar = torch.cat([rbar, ubar], dim=0).contiguous()
         if rbar is None and self._jit_usable(n):   # the problem's own forward kernel (programs compiled in): jit.py
             _check(self.lib.pj_forward_train_jit(self._jit.function, ctypes.byref(self.spec), prog.data_ptr(), prog_len,
@@ -499,8 +538,8 @@ class FusedProblem:
                                                  self.workspace.data_ptr(), self.workspace.numel(), self._stream()),
                    "pj_forward_train_jit")
         else:
-            _check(self.lib.pj_forward_train(ctypes.byref(self.spec), prog.data_ptr(), prog_len, *self._prog_w_args(), ptrs, n,
-                                             self.pack_buf.data_ptr(), ctypes.c_float(scale),
+            _check(self._fn("pj_forward_train")(ctypes.byref(self.spec), prog.data_ptr(), prog_len, *self._prog_w_args(), ptrs, n,
+                                                self.pack_buf.data_ptr(), (ctypes.c_double if self.f64 else ctypes.c_float)(scale),
                                              rbar.data_ptr() if rbar is not None else None,
                                              r.data_ptr() if want_residual else None, sumsq_out.data_ptr(),
                                              self.workspace.data_ptr(), self.workspace.numel(), self._stream()),
@@ -511,14 +550,14 @@ class FusedProblem:
             raise ValueError("residual_grad(reducer=...) sums self.gradbuf: pass sumsq_out=self.sumsq")
         if reducer is not None and getattr(reducer, "n", self.gradbuf.numel()) != self.gradbuf.numel():
             raise ValueError("residual_grad(reducer=...): the reducer was built for a buffer of another size than gradbuf")
-        if reducer is not None and reducer.fused_args is not None:
+        if reducer is not None and reducer.fused_args is not None and not self.f64:   # the fused collective is float only
             peers, rank, world = reducer.fused_args
             _check(self.lib.pj_backward_allreduce(ctypes.byref(self.spec), ptrs, n, self.pack_buf.data_ptr(),
                                                   self.gradbuf.data_ptr(), self.gradbuf.numel() - self.grad.numel(),
                                                   self.workspace.data_ptr(), self.workspace.numel(), peers, rank, world,
                                                   self._stream()), "pj_backward_allreduce")
         else:
-            _check(self.lib.pj_backward(ctypes.byref(self.spec), ptrs, n, self.pack_buf.data_ptr(), self.grad.data_ptr(),
+            _check(self._fn("pj_backward")(ctypes.byref(self.spec), ptrs, n, self.pack_buf.data_ptr(), self.grad.data_ptr(),
                                         self.workspace.data_ptr(), self.workspace.numel(), self._stream()), "pj_backward")
             if reducer is not None:
                 reducer(self.gradbuf)
@@ -533,6 +572,8 @@ class FusedProblem:
         if self._jit is not None:
             return True
         try:
+            if self.f64:
+                raise ValueError("the specialised kernel is float32 only (this problem runs in float64)")
             if self._patch_sets:
                 raise ValueError("the program has trainable immediates (Resnet shortcut)")
             if not self.plan_info(1024)["tc"]:
@@ -561,7 +602,7 @@ class FusedProblem:
         n = 19 + PJ_MAX_NETS * (2 * PJ_MAX_LINEAR + 1) + 6
         out = (ctypes.c_int64 * n)()
         with torch.cuda.device(self.device):
-            _check(self.lib.pj_plan_info(ctypes.byref(self.spec), n_points, out, n), "pj_plan_info")
+            _check(self._fn("pj_plan_info")(ctypes.byref(self.spec), n_points, out, n), "pj_plan_info")
         keys = ("T P Q C RS n_tiles grid hmax n_stage_fwd n_stage_bwd resident_fwd resident_bwd zj_tile_floats ws_zj "
                 "ws_seed ws_gpart ws_bytes smem_fwd smem_bwd").split()
         info = {k: int(out[i]) for i, k in enumerate(keys)}
@@ -600,8 +641,8 @@ class FusedProblem:
         if getattr(self, "_graph_keys_seen", 0) >= self.GRAPH_MAX_DISTINCT:
             return None                                    # ever-changing batch sizes: plain launches from here on
         dev = self.device
-        static = [torch.zeros(n, dtype=torch.float32, device=dev) for _ in range(self.n_coords)]
-        stage = _PinnedStage(self.n_coords, n, dev)
+        static = [torch.zeros(n, dtype=self.dtype, device=dev) for _ in range(self.n_coords)]
+        stage = _PinnedStage(self.n_coords, n, dev, self.dtype)
 
         def body():
             if train:
@@ -631,7 +672,7 @@ class FusedProblem:
             src = src.detach().reshape(-1)
             if src.device.type != "cpu":
                 dst.copy_(src)
-            elif src.is_pinned() and src.dtype == torch.float32 and src.is_contiguous():
+            elif src.is_pinned() and src.dtype == dst.dtype and src.is_contiguous():
                 dst.copy_(src, non_blocking=True)     # already page-locked: DMA straight from the caller's buffer
             else:
                 stage.copy_in(i, dst, src)
@@ -647,7 +688,7 @@ class FusedProblem:
         zero_gradbuf = bool(zero_gradbuf and train)
         st = self._graph_state(n, n_glob, train, zero_gradbuf)
         if st is None:                                  # graph cache exhausted (see GRAPH_MAX_DISTINCT): eager launches
-            dev_coords = [c.detach().reshape(-1).to(self.device, torch.float32) for c in coords]
+            dev_coords = [c.detach().reshape(-1).to(self.device, self.dtype) for c in coords]
             if train:
                 self.residual_grad(dev_coords, n_global=n_glob, sumsq_out=self.sumsq, zero_gradbuf=zero_gradbuf)
             else:
@@ -666,14 +707,16 @@ class FusedProblem:
         Not used by the solvers yet; single rank only."""
         if not getattr(optimizer, "capturable", False):
             raise ValueError("train_step_graphed needs FlatAdam(..., capturable=True)")
+        if self.f64:
+            raise ValueError("train_step_graphed: FlatAdam (pj_adam_step) is float32 only")
         n = coords[0].numel()
         n_glob = n if n_global is None else n_global
         key = ("step", int(n), int(n_glob), id(optimizer))
         st = self._graph_lookup(key)
         if st is None:
             dev = self.device
-            static = [torch.zeros(n, dtype=torch.float32, device=dev) for _ in range(self.n_coords)]
-            stage = _PinnedStage(self.n_coords, n, dev)
+            static = [torch.zeros(n, dtype=self.dtype, device=dev) for _ in range(self.n_coords)]
+            stage = _PinnedStage(self.n_coords, n, dev, self.dtype)
 
             def body():
                 self.gradbuf.zero_()

@@ -29,10 +29,11 @@ def all_reduce_gradbuf(gradbuf, dist=None):
 
 
 class GradBufReducer:
-    """SUM of one flat float32 buffer over the ranks, in place; ``mode`` says how: ``"single"`` (no process group),
+    """SUM of one flat float32 (or float64) buffer over the ranks, in place; ``mode`` says how: ``"single"`` (no process group),
     ``"oneshot-nvlink"`` (one launch of ``pj_allreduce_oneshot``: every rank reads its peers' copies over NVLink and adds
     them in rank order -- bit-identical results everywhere, CUDA-graph capturable) or ``"process-group"``
-    (``dist.all_reduce``).  ``PINNJET_ALLREDUCE=nccl`` forces the last one.
+    (``dist.all_reduce``).  ``PINNJET_ALLREDUCE=nccl`` forces the last one, and so does a float64 buffer: the NVLink
+    collectives push 64-bit {epoch, float32} words.
 
     ``fused_args`` (one-shot mode only, else ``None``): ``(peer pointers, rank, world)`` of a SECOND symmetric buffer, for
     ``pj_backward_allreduce`` -- the reverse kernel's partial reduction and this collective as one launch
@@ -47,6 +48,9 @@ class GradBufReducer:
         world = dist.get_world_size()
         if not buf.is_cuda:
             self.why = "buffer not on a GPU"
+            return
+        if buf.dtype == torch.float64:
+            self.why = "float64 buffer (the NVLink collectives are float32 only)"
             return
         if os.environ.get("PINNJET_ALLREDUCE", "").lower() in ("nccl", "process-group"):
             self.why = "PINNJET_ALLREDUCE"
@@ -87,13 +91,13 @@ class GradBufReducer:
             self.why = f"{type(exc).__name__}: {exc}"
 
     def __call__(self, buf):
-        if self.mode == "oneshot-nvlink":
+        if self.mode == "oneshot-nvlink" and buf.dtype != torch.float64:
             if buf.numel() != self._n or buf.dtype != torch.float32 or not buf.is_contiguous():
                 raise ValueError("GradBufReducer: buffer does not match the one it was built for")
             rc = self._lib.pj_allreduce_oneshot(self._ptrs, self._rank, self._world, buf.data_ptr(), buf.data_ptr(), self._n,
                                                 ctypes.c_void_p(torch.cuda.current_stream(buf.device).cuda_stream))
             if rc != 0:
                 raise RuntimeError(f"pj_allreduce_oneshot failed ({rc})")
-        elif self.mode == "process-group":
+        elif self.mode != "single":
             self.dist.all_reduce(buf)
         return buf

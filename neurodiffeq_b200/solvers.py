@@ -26,7 +26,7 @@ import torch
 import torch.nn as nn
 
 from .conditions import BaseCondition
-from .engine import FusedProblem
+from .engine import FusedProblem, check_dtype
 from .eager import build_problem
 from ._compat import renamed_arguments
 from .losses import _losses, h1_rows, h1_semi_rows
@@ -70,7 +70,7 @@ def _unique(params):
 class BaseSolution:
     """Callable solution ``u(*coords)`` evaluated by the forward kernel (reference solvers.py:650-720)."""
 
-    def __init__(self, nets, conditions, n_coords, coords_for_condition=None, enforce=None, device=None):
+    def __init__(self, nets, conditions, n_coords, coords_for_condition=None, enforce=None, device=None, dtype=None):
         if nets is None:
             raise RuntimeError("The nets cannot be None, check if you disabled validation "
                                "and used `best`=True with `get_solution` / `get_residual`")
@@ -80,13 +80,14 @@ class BaseSolution:
         self._cfc = coords_for_condition
         self._enforce = enforce
         self._device = device
+        self._dtype_kw = {"dtype": torch.float64} if check_dtype(dtype) == torch.float64 else {}
         self._problem = None
 
     def _fused(self):
         if self._problem is None:
             # the fused forward kernel, or the autograd path for what the tracer refuses (eager.py)
             self._problem = build_problem(FusedProblem, self.nets, self.conditions, None, self._n_coords, self._cfc,
-                                          device=self._device, enforce=self._enforce)
+                                          device=self._device, enforce=self._enforce, **self._dtype_kw)
         return self._problem
 
     @renamed_arguments(as_type="to_numpy")                          # reference solvers.py:681
@@ -111,7 +112,11 @@ class BaseSolution:
 
 
 class BaseSolver:
-    """Fused counterpart of ``neurodiffeq.solvers.BaseSolver``."""
+    """Fused counterpart of ``neurodiffeq.solvers.BaseSolver``.
+
+    ``dtype``: ``None`` or ``torch.float32`` (the default) trains in float32; ``torch.float64`` -- the reference's precision
+    -- converts the networks to float64 and runs the double kernels (or the autograd path in float64 for what the fused
+    engine refuses).  The device loop, ``optim.FlatAdam`` and the specialised kernel stay float32 only."""
 
     N_COORDS = None  # set by subclasses that know it a priori
 
@@ -119,7 +124,9 @@ class BaseSolver:
     def __init__(self, diff_eqs, conditions, nets=None, train_generator=None, valid_generator=None,
                  analytic_solutions=None, optimizer=None, loss_fn=None, n_batches_train=1, n_batches_valid=4,
                  metrics=None, n_input_units=None, n_output_units=None, shuffle=None, batch_size=None,
-                 device=None, data_parallel=True, device_loop=False, jit=None):
+                 device=None, data_parallel=True, device_loop=False, jit=None, dtype=None):
+        self.dtype = check_dtype(dtype)
+        dtype_kw = {"dtype": torch.float64} if self.dtype == torch.float64 else {}   # the float32 path is called as before
         if shuffle:
             warnings.warn("param `shuffle` is deprecated and ignored; shuffling should be performed by generators",
                           FutureWarning)
@@ -168,7 +175,7 @@ class BaseSolver:
             self.problem = build_problem(FusedProblem, self.nets, self.conditions,
                                          h1_semi_rows(self._traced_diff_eqs, self.n_funcs),
                                          n_coords, coords_for_condition=self._coords_for_condition, device=device,
-                                         aux_outputs=self._traced_diff_eqs, enforce=self.compute_func_val)
+                                         aux_outputs=self._traced_diff_eqs, enforce=self.compute_func_val, **dtype_kw)
             self.n_eq = len(self.problem.tp.aux_rows)
         else:
             # the fused engine (trace once -> kernels); what its tracer / planner refuses runs on the autograd path with one
@@ -176,7 +183,7 @@ class BaseSolver:
             self.problem = build_problem(FusedProblem, self.nets, self.conditions,
                                          self._h1_rows if self._h1 else self._traced_diff_eqs, n_coords,
                                          coords_for_condition=self._coords_for_condition, device=device,
-                                         enforce=self.compute_func_val)
+                                         enforce=self.compute_func_val, **dtype_kw)
             self.n_eq = self.problem.n_eq - (n_coords if self._h1 else 0)     # the user's equations
         self.device = self.problem.device
         # The residual programs compiled INTO the forward kernel (jit.py: ~1 s of nvcc per problem, cached on disk; identical
@@ -207,7 +214,7 @@ class BaseSolver:
         # an epoch replay as ONE CUDA graph; losses stay on the device and are read back in bulk (see _fit_device_loop).
         self.device_loop = bool(device_loop)
         self._device_loop_state = None
-        if self.device_loop and optimizer is None:   # the reference default (Adam, lr 1e-3) on the flat buffers, capturable
+        if self.device_loop and optimizer is None and self.dtype == torch.float32:   # the reference default (Adam, lr 1e-3) on the flat buffers, capturable
             from .optim import FlatAdam
             self.optimizer = FlatAdam(self.problem.theta, self.problem.grad, capturable=True)
 
@@ -342,7 +349,7 @@ class BaseSolver:
         return cols
 
     def _to_device(self, cols):
-        return [c.to(self.device, torch.float32, non_blocking=True).contiguous() for c in cols]
+        return [c.to(self.device, self.dtype, non_blocking=True).contiguous() for c in cols]
 
     def _update_history(self, value, metric_type, key):
         self._phase = key
@@ -435,7 +442,7 @@ class BaseSolver:
             return self._run_train_epoch_with_closure()
         metric_values = {name: 0.0 for name in self.metrics_fn}
         n_b = self.n_batches[key]
-        loss_acc = torch.zeros(1, dtype=torch.float32, device=self.device)
+        loss_acc = torch.zeros(1, dtype=self.dtype, device=self.device)
         # parameters changed at the last optimizer step: K0 re-packs them and, for a training phase, clears [grad | sum r^2]
         # in the same launch (optimizer.zero_grad(): the kernels accumulate into the p.grad views)
         fp.pack(zero_gradbuf=(key == "train"))
@@ -462,7 +469,7 @@ class BaseSolver:
                     loss.backward()                                          # only to get dL/dr, dL/du on the tiny leaves
                     fp.residual_grad(coords, rbar=_grad_or_zeros(res).t().contiguous(), ubar=u.grad, sumsq_out=fp.sumsq,
                                      repack=False)
-                loss_acc += loss.detach().reshape(1).to(torch.float32)
+                loss_acc += loss.detach().reshape(1).to(self.dtype)
             self._eval_metrics(coords, metric_values)
         if self._dist is not None:   # one collective per epoch phase: [grad | loss] summed over the ranks
             fp.sumsq.copy_(loss_acc)
@@ -525,6 +532,8 @@ class BaseSolver:
         """None if an epoch of this solver can run as one captured graph, else the reason it cannot."""
         from .device_sampling import describe
         from .optim import FlatAdam
+        if self.dtype == torch.float64:
+            return "device sampling and optim.FlatAdam are float32 only; this solver trains in float64"
         if getattr(self.problem, "is_eager", False):
             return "the problem runs on the autograd path (" + self.problem.reason + ")"
         if self._custom_loss is not None:
@@ -677,7 +686,8 @@ class BaseSolver:
 
     def get_solution(self, copy=True, best=True):
         return self._solution(copy, best, lambda nets, conditions: self._solution_class()(
-            nets, conditions, self.n_coords, self._coords_for_condition, enforce=self.compute_func_val, device=self.device))
+            nets, conditions, self.n_coords, self._coords_for_condition, enforce=self.compute_func_val, device=self.device,
+            dtype=self.dtype))
 
     def _solution(self, copy, best, make):
         """``make(nets, conditions)`` on the best or live networks, copied unless ``copy=False``."""
@@ -759,8 +769,8 @@ class SolutionSphericalHarmonics(SolutionSpherical):
     kernel evaluates it.  ``max_degree`` is deprecated: it selects ``RealSphericalHarmonics(max_degree)`` unless
     ``harmonics_fn`` is given."""
 
-    def __init__(self, nets, conditions, max_degree=None, harmonics_fn=None, device=None):
-        super().__init__(nets, conditions, 3, enforce=self._compute_u, device=device)
+    def __init__(self, nets, conditions, max_degree=None, harmonics_fn=None, device=None, dtype=None):
+        super().__init__(nets, conditions, 3, enforce=self._compute_u, device=device, dtype=dtype)
         if harmonics_fn is None and max_degree is None:
             raise ValueError("harmonics_fn should be specified")
         if max_degree is not None:
@@ -892,7 +902,7 @@ class SolverSpherical(BaseSolver):
         if harmonics_fn is None:
             return super().get_solution(copy=copy, best=best)
         return self._solution(copy, best, lambda nets, conditions: SolutionSphericalHarmonics(
-            nets, conditions, harmonics_fn=harmonics_fn, device=self.device))
+            nets, conditions, harmonics_fn=harmonics_fn, device=self.device, dtype=self.dtype))
 
     def _get_internal_variables(self):
         d = super()._get_internal_variables()

@@ -30,6 +30,7 @@ OP_SIN, OP_COS, OP_EXP, OP_LOG, OP_TANH, OP_SQRT, OP_ABS, OP_SIGN, OP_POWC, OP_R
 OP_ST_U, OP_ST_R, OP_ST_SEED = 20, 21, 22
 OP_TAN, OP_SINH, OP_COSH, OP_ATAN, OP_ERF = 23, 24, 25, 26, 27
 OP_ST_W = 28   # store a per-point weight of the combined second-order channel
+OP_POW = 29    # slot ** slot: double programs only (an exponent float32 cannot hold, Program.to_f64)
 
 _UNARY = {"neg": OP_NEG, "sin": OP_SIN, "cos": OP_COS, "exp": OP_EXP, "log": OP_LOG, "tanh": OP_TANH,
           "sqrt": OP_SQRT, "abs": OP_ABS, "sign": OP_SIGN, "rcp": OP_RCP, "tan": OP_TAN, "sinh": OP_SINH,
@@ -1041,18 +1042,57 @@ class ChannelScheme:
 class Program:
     """Lowered bytecode: int32 array [len, 4]  (op, dst, a, b)  -- see csrc/pinnjet_program.cuh."""
 
-    def __init__(self, code, n_slots, exact_imm=None, patch=None):
+    def __init__(self, code, n_slots, exact_imm=None, patch=None, f64=False):
         self.code = np.asarray(code, dtype=np.int32).reshape(-1, 4)
         self.n_slots = n_slots
         self.exact_imm = exact_imm or {}  # instruction index -> float64 immediate (host-side checks only)
         self.patch = patch or {}          # instruction index -> key of the trainable scalar its immediate must hold
+        self.f64 = f64                    # lowering for the double kernels (see to_f64)
 
     def __len__(self):
         return self.code.shape[0]
 
+    def to_f64(self):
+        """The program for the double kernels, with every immediate the exact double the host traced: OP_CONST holds the
+        double's low word in ``a`` and its high word in ``b`` (patched constants: both words); an OP_POWC exponent
+        float32 cannot hold exactly becomes OP_CONST into a fresh slot + OP_POW (two slots, double programs only).
+        The float program is left as it is."""
+        if self.f64:
+            return self
+        code, exact, patch, extra = [], {}, {}, self.n_slots
+        for pc, (op, dst, a, b) in enumerate(self.code.tolist()):
+            if op == OP_CONST:
+                if pc in self.patch:
+                    patch[len(code)] = self.patch[pc]
+                    lo = hi = 0
+                else:
+                    v = self.exact_imm.get(pc, float(np.int32(a).view(np.float32)))
+                    exact[len(code)] = v
+                    lo, hi = _f64_words(v)
+                code.append((OP_CONST, dst, lo, hi))
+            elif op == OP_POWC and pc in self.exact_imm and float(np.float32(self.exact_imm[pc])) != self.exact_imm[pc]:
+                exact[len(code)] = self.exact_imm[pc]
+                code.append((OP_CONST, extra, *_f64_words(self.exact_imm[pc])))
+                code.append((OP_POW, dst, a, extra))
+            else:
+                if op == OP_POWC and pc in self.exact_imm:
+                    exact[len(code)] = self.exact_imm[pc]
+                code.append((op, dst, a, b))
+        n_slots = extra + 1 if any(c[0] == OP_POW for c in code) else self.n_slots
+        return Program(code, n_slots, exact, patch, f64=True)
+
 
 def _f32_bits(v):
     return int(np.array([v], dtype=np.float32).view(np.int32)[0])
+
+
+def _f64_words(v):
+    lo, hi = np.array([v], dtype=np.float64).view(np.int32).tolist()   # little endian: low word first
+    return lo, hi
+
+
+def _f64_of_words(lo, hi):
+    return float(np.array([lo, hi], dtype=np.int32).view(np.float64)[0])
 
 
 def lower(outputs, yrow_of):
@@ -1122,7 +1162,8 @@ def depends_on_jets(expr):
 
 def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n_seed=0, n_w=0, theta=None):
     """Pure-numpy interpreter of the bytecode (host-side check of the lowering; float64).  ``theta``: values of the
-    trainable scalars the program's patched constants stand for (``Program.patch`` keys -> float)."""
+    trainable scalars the program's patched constants stand for (``Program.patch`` keys -> float).  Float programs take
+    their immediates from ``exact_imm``; double programs (``Program.to_f64``) are decoded from the code alone."""
     n = coords.shape[1]
     val = np.zeros((program.n_slots, n))
     u, r, seed = np.zeros((n_u, n)), np.zeros((n_r, n)), np.zeros((n_seed, n))
@@ -1133,7 +1174,10 @@ def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n
           OP_SINH: np.sinh, OP_COSH: np.cosh, OP_ATAN: np.arctan}
     for pc, (op, dst, a, b) in enumerate(program.code.tolist()):
         if op == OP_CONST:
-            val[dst] = theta[program.patch[pc]] if pc in program.patch else program.exact_imm.get(pc, bits(a))
+            if pc in program.patch:
+                val[dst] = theta[program.patch[pc]]
+            else:
+                val[dst] = _f64_of_words(a, b) if program.f64 else program.exact_imm.get(pc, bits(a))
         elif op == OP_COORD:
             val[dst] = coords[a]
         elif op == OP_NET:
@@ -1151,7 +1195,9 @@ def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n
         elif op == OP_DIV:
             val[dst] = val[a] / val[b]
         elif op == OP_POWC:
-            val[dst] = val[a] ** program.exact_imm.get(pc, bits(b))
+            val[dst] = val[a] ** (bits(b) if program.f64 else program.exact_imm.get(pc, bits(b)))
+        elif op == OP_POW:
+            val[dst] = val[a] ** val[b]
         elif op == OP_ERF:
             from scipy.special import erf
             val[dst] = erf(val[a])
