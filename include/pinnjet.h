@@ -52,7 +52,8 @@ typedef struct PjNet {
     int32_t n_linear;                   /* number of nn.Linear layers (>= 2)                                  */
     int32_t width[PJ_MAX_LINEAR + 1];   /* width[0]=n_in, width[l]=out_features of Linear l-1                 */
     int32_t act;                        /* PJ_ACT_*                                                           */
-    int32_t yrow0;                      /* first row of this net in the jet table: row = yrow0 + o*C + c      */
+    int32_t yrow0;                      /* first row of this net in the jet table: row = yrow0 + o*C + c,     */
+                                        /* C = 1 + n1 + n2 + n3                                               */
     int64_t w_off[PJ_MAX_LINEAR];       /* float offset of W_l (torch layout [out][in]) in theta / grad_theta */
     int64_t b_off[PJ_MAX_LINEAR];       /* float offset of b_l                                                */
 } PjNet;
@@ -63,6 +64,7 @@ typedef struct PjSpec {
     int32_t n_coords;                   /* number of sampled coordinates (d0)                                 */
     int32_t n_nets;                     /* distinct networks                                                  */
     int32_t n1, n2;                     /* jet channels: value | n1 directional firsts | n2 second-order      */
+                                        /* (| n3 pure thirds: see n3 at the end)                              */
     int32_t wl;                         /* 0: the n2 channels are pure seconds of the first n2 directions;    */
                                         /* >0: n2 == 1 and the channel is L = sum_{d<wl} w_d(x) D_d^2 with    */
                                         /* per-point weights produced by the weight program (prog_w)          */
@@ -72,6 +74,9 @@ typedef struct PjSpec {
     int32_t n_slots;                    /* value-file size the programs need                                  */
     int64_t n_theta;                    /* floats in theta                                                    */
     PjNet net[PJ_MAX_NETS];
+    int32_t n3;                         /* pure third-order channels of the first n3 directions, after the    */
+                                        /* n2 channels (n3 <= n2, wl == 0); 0: none.  Appended last, so a     */
+                                        /* zero-initialised spec of an older caller means what it meant       */
 } PjSpec;
 
 /* Sizes the caller needs to allocate buffers (all bytes; workspace contents are opaque). */

@@ -9,6 +9,8 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SCHEMES = [(1, 0, 0), (1, 1, 0), (2, 0, 0), (2, 1, 0), (2, 2, 0), (3, 0, 0), (3, 3, 0), (2, 1, 2), (3, 1, 3), (4, 1, 4)]
+# (n1, n2, wl, n3): schemes with pure third-order channels (PjSpec.n3).  FFMA kernels only, float and double.
+THIRD_ORDER_SCHEMES = [(1, 1, 0, 1), (2, 1, 0, 1)]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
@@ -53,6 +55,11 @@ def build(force=False, verbose=False, extra_flags=(), lib=None, objdir_name="bui
             jobs.append((os.path.join(objdir, f"inst_{n1}_{n2}_{wl}" + ("_f64" if f64 else "") + ".o"),
                          os.path.join(HERE, "pinnjet_inst.cu"),
                          [f"-DPJ_N1={n1}", f"-DPJ_N2={n2}", f"-DPJ_WL={wl}", f"-DPJ_F64={f64}"] + list(extra_flags)))
+    for n1, n2, wl, n3 in THIRD_ORDER_SCHEMES:
+        for f64 in (0, 1):
+            jobs.append((os.path.join(objdir, f"inst_{n1}_{n2}_{wl}_{n3}" + ("_f64" if f64 else "") + ".o"),
+                         os.path.join(HERE, "pinnjet_inst.cu"),
+                         [f"-DPJ_N1={n1}", f"-DPJ_N2={n2}", f"-DPJ_WL={wl}", f"-DPJ_N3={n3}", f"-DPJ_F64={f64}"] + list(extra_flags)))
     logs = []
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         for out, rc, log in ex.map(_compile, jobs):

@@ -31,6 +31,8 @@ PJ_DECL(3, 3, 0)
 PJ_DECL(2, 1, 2)   // combined second-order channel over 2 / 3 weighted directions
 PJ_DECL(3, 1, 3)
 PJ_DECL(4, 1, 4)   // 4 directions (e.g. x, t, a boundary abscissa and one polarisation direction), combined only
+PJ_DECL(1, 1, 0_1) // pure third-order channels (PjSpec.n3 = 1): u''' of ODEs, u_xxx of 1-D evolution equations
+PJ_DECL(2, 1, 0_1)
 #undef PJ_DECL
 cudaError_t launch_reduce(const float* gpart, int n_parts, long long n_theta, float* grad, cudaStream_t s);
 cudaError_t launch_reduce_f64(const double* gpart, int n_parts, long long n_theta, double* grad, cudaStream_t s);
@@ -49,19 +51,20 @@ template <> struct Kernels<double> {
     int (*occ)(const Plan&, int, int);
 };
 struct SchemeEntry {
-    int n1, n2, wl;
+    int n1, n2, wl, n3;
     Kernels<float> f32;
     Kernels<double> f64;
     template <typename R> const Kernels<R>& of() const;
 };
 template <> const Kernels<float>& SchemeEntry::of<float>() const { return f32; }
 template <> const Kernels<double>& SchemeEntry::of<double>() const { return f64; }
-#define PJ_ENTRY(N1, N2, WL)                                                                                                  \
-    {N1, N2, WL, {launch_k1_##N1##_##N2##_##WL, launch_k2_##N1##_##N2##_##WL, occupancy_##N1##_##N2##_##WL},                   \
-     {launch_k1_f64_##N1##_##N2##_##WL, launch_k2_f64_##N1##_##N2##_##WL, occupancy_f64_##N1##_##N2##_##WL}}
+#define PJ_ENTRY(N1, N2, WL, N3, NAME)                                                                                        \
+    {N1, N2, WL, N3, {launch_k1_##NAME, launch_k2_##NAME, occupancy_##NAME},                                                  \
+     {launch_k1_f64_##NAME, launch_k2_f64_##NAME, occupancy_f64_##NAME}}
 static const SchemeEntry kSchemes[] = {
-    PJ_ENTRY(1, 0, 0), PJ_ENTRY(1, 1, 0), PJ_ENTRY(2, 0, 0), PJ_ENTRY(2, 1, 0), PJ_ENTRY(2, 2, 0),
-    PJ_ENTRY(3, 0, 0), PJ_ENTRY(3, 3, 0), PJ_ENTRY(2, 1, 2), PJ_ENTRY(3, 1, 3), PJ_ENTRY(4, 1, 4),
+    PJ_ENTRY(1, 0, 0, 0, 1_0_0), PJ_ENTRY(1, 1, 0, 0, 1_1_0), PJ_ENTRY(2, 0, 0, 0, 2_0_0), PJ_ENTRY(2, 1, 0, 0, 2_1_0),
+    PJ_ENTRY(2, 2, 0, 0, 2_2_0), PJ_ENTRY(3, 0, 0, 0, 3_0_0), PJ_ENTRY(3, 3, 0, 0, 3_3_0), PJ_ENTRY(2, 1, 2, 0, 2_1_2),
+    PJ_ENTRY(3, 1, 3, 0, 3_1_3), PJ_ENTRY(4, 1, 4, 0, 4_1_4), PJ_ENTRY(1, 1, 0, 1, 1_1_0_1), PJ_ENTRY(2, 1, 0, 1, 2_1_0_1),
 };
 #undef PJ_ENTRY
 
@@ -74,9 +77,9 @@ static int fail(int code, const char* fmt, ...) {
     return code;
 }
 
-static const SchemeEntry* find_scheme(int n1, int n2, int wl) {
+static const SchemeEntry* find_scheme(const PjSpec& sp) {
     for (const auto& e : kSchemes)
-        if (e.n1 == n1 && e.n2 == n2 && e.wl == wl) return &e;
+        if (e.n1 == sp.n1 && e.n2 == sp.n2 && e.wl == sp.wl && e.n3 == sp.n3) return &e;
     return nullptr;
 }
 
@@ -89,14 +92,14 @@ static const SchemeEntry* find_scheme(int n1, int n2, int wl) {
 
 template <typename R>
 static int occupancy(const PjSpec& sp, const Plan& pl, int k, int smem) {
-    return find_scheme(sp.n1, sp.n2, sp.wl)->of<R>().occ(pl, k, smem);
+    return find_scheme(sp)->of<R>().occ(pl, k, smem);
 }
 
 // make_plan (pinnjet_plan.cpp) for the current device, the current value of PINNJET_TC and the kernels of element type R
 template <typename R = float>
 static int device_plan(const PjSpec& sp, long long N, int prog_len, Plan& pl, int prog_w_len = 0) {
-    if (!find_scheme(sp.n1, sp.n2, sp.wl))
-        return fail(-2, "jet channel scheme (n1=%d, n2=%d, wl=%d) has no compiled kernel", sp.n1, sp.n2, sp.wl);
+    if (!find_scheme(sp))
+        return fail(-2, "jet channel scheme (n1=%d, n2=%d, wl=%d, n3=%d) has no compiled kernel", sp.n1, sp.n2, sp.wl, sp.n3);
     PlanDevice dev = {0, PJ_TC_DEFAULT, occupancy<R>};
     int d = 0;
     if (cudaGetDevice(&d) != cudaSuccess || cudaDeviceGetAttribute(&dev.sms, cudaDevAttrMultiProcessorCount, d) != cudaSuccess)
@@ -359,7 +362,7 @@ static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, con
     a.zj = mode == 1 ? reinterpret_cast<R*>(w + (a.plan.tc ? a.plan.ws_tcrec : a.plan.ws_zj)) : nullptr;
     a.seeds = mode == 1 ? reinterpret_cast<R*>(w + a.plan.ws_seed) : nullptr;
     a.wts = mode == 1 ? reinterpret_cast<R*>(w + a.plan.ws_wts) : nullptr;
-    const SchemeEntry* e = find_scheme(spec->n1, spec->n2, spec->wl);
+    const SchemeEntry* e = find_scheme(*spec);
     if (jit_function) {   // the problem's own forward kernel: same arguments, same plan
         if (!a.plan.tc) return fail(-2, "the specialised forward kernel exists for the tensor-core path only");
         CuLaunchKernelEx launch = cu_launch_kernel_ex();
@@ -456,7 +459,7 @@ static int run_k2(const PjSpec* spec, const R* const* coords, int64_t n_points, 
     a.gpart = reinterpret_cast<R*>(w + a.plan.ws_gpart);
     a.wts = reinterpret_cast<const R*>(w + a.plan.ws_wts);
     a.dbg = reinterpret_cast<float*>(w + a.plan.ws_loss) + LOSS_DBG_WORD;
-    const SchemeEntry* e = find_scheme(spec->n1, spec->n2, spec->wl);
+    const SchemeEntry* e = find_scheme(*spec);
     if (int rc = check_cuda(e->of<R>().k2(a, a.plan.grid_bwd, a.plan.k2_bytes, (cudaStream_t)stream), "backward launch")) return rc;
     *gpart = a.gpart;
     *n_parts = a.plan.grid_bwd;

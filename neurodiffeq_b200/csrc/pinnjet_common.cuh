@@ -280,7 +280,8 @@ __device__ __forceinline__ R pg_reduce_scatter4(const R (&v)[4], int pg_lane) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// activation jets (SURVEY.md Appendix A).  Channels: 0 value | 1..N1 first order | N1+1..N1+N2 pure second order.
+// activation jets (SURVEY.md Appendix A).  Channels: 0 value | 1..N1 first order | N1+1..N1+N2 pure second order |
+// N1+N2+1..N1+N2+N3 pure third order of the first N3 directions.
 // ---------------------------------------------------------------------------------------------------------------------
 // Branch-free tanh, ~1-4 ulp: |x| < 0.6: x + x^3 P(x^2) (degree-4 minimax fit, 1.4 ulp); else 1 - 2/(exp(2|x|)+1) with
 // ex2.approx / rcp.approx.  Straight-line code: the 8-16 independent calls of an activation epilogue pipeline instead of
@@ -325,10 +326,21 @@ __device__ __forceinline__ void sincos_r(float x, float* s, float* c) { sincosf(
 __device__ __forceinline__ void sincos_r(double x, double* s, double* c) { sincos(x, s, c); }
 
 // z-jet -> a-jet, in place.  WL > 0: the single second-order channel is the weighted combination L = sum_d w[d] D_d^2.
-template <int N1, int N2, int WL, typename R>
-__device__ __forceinline__ void act_forward(int act, R (&z)[1 + N1 + N2], const R* w) {
+// N3 > 0: channels 1+N1+N2+t (t < N3) are the pure thirds of direction t, a3 = s3 z1^3 + 3 s2 z1 z2 + s1 z3 (N3 <= N2:
+// direction t has its first and second channel).
+template <int N1, int N2, int WL, int N3, typename R>
+__device__ __forceinline__ void act_forward(int act, R (&z)[1 + N1 + N2 + N3], const R* w) {
     R a0, s1, s2;
     act_d2(act, z[0], a0, s1, s2);
+    if constexpr (N3 > 0) {   // before the first- and second-order channels are overwritten
+        static_assert(WL == 0 && N3 <= N2, "third-order channels need the pure second of their direction");
+        const R s3 = act == PJ_ACT_TANH ? R(-2) * s1 * s1 - R(2) * a0 * s2 : -s1;
+#pragma unroll
+        for (int t = 0; t < N3; ++t) {
+            const R z1 = z[1 + t], z2 = z[1 + N1 + t];
+            z[1 + N1 + N2 + t] = fma(s3 * z1 * z1, z1, fma(R(3) * s2 * z1, z2, s1 * z[1 + N1 + N2 + t]));
+        }
+    }
     if constexpr (WL > 0) {
         static_assert(N2 == 1, "combined mode carries one second-order channel");
         R q = 0.0f;
@@ -347,9 +359,9 @@ __device__ __forceinline__ void act_forward(int act, R (&z)[1 + N1 + N2], const 
 // reverse of the activation jet: given the stored record (channel 0 = tanh(z0) for tanh nets, z0 for sin nets; other
 // channels z-jets) and the adjoint of the a-jet, produce the a-jet (for the weight-gradient GEMM) and the adjoint of the
 // z-jet.
-template <int N1, int N2, int WL, typename R>
-__device__ __forceinline__ void act_backward(int act, const R (&z)[1 + N1 + N2], const R (&ab)[1 + N1 + N2],
-                                             R (&a)[1 + N1 + N2], R (&zb)[1 + N1 + N2], const R* w) {
+template <int N1, int N2, int WL, int N3, typename R>
+__device__ __forceinline__ void act_backward(int act, const R (&z)[1 + N1 + N2 + N3], const R (&ab)[1 + N1 + N2 + N3],
+                                             R (&a)[1 + N1 + N2 + N3], R (&zb)[1 + N1 + N2 + N3], const R* w) {
     R a0, s1, s2, s3;
     if (act == PJ_ACT_TANH) {   // record channel 0 = tanh(z0), stored by K1: no transcendental in the reverse pass
         a0 = z[0];
@@ -388,6 +400,19 @@ __device__ __forceinline__ void act_backward(int act, const R (&z)[1 + N1 + N2],
             zb[1 + s] = fma(R(2) * s2 * zf, abs_, zb[1 + s]);
             zb0 = fma(fma(s3 * zf, zf, s2 * zs), abs_, zb0);
             a[1 + N1 + s] = fma(s2 * zf, zf, s1 * zs);
+        }
+    }
+    if constexpr (N3 > 0) {   // reverse of a3 = s3 z1^3 + 3 s2 z1 z2 + s1 z3; s4 from the stored tanh(z0) or sin(z0)
+        const R s4 = act == PJ_ACT_TANH ? R(-6) * s1 * s2 - R(2) * a0 * s3 : a0;
+#pragma unroll
+        for (int t = 0; t < N3; ++t) {
+            const R z1 = z[1 + t], z2 = z[1 + N1 + t], z3 = z[1 + N1 + N2 + t], ab3 = ab[1 + N1 + N2 + t];
+            const R z1s = z1 * z1;
+            zb[1 + N1 + N2 + t] = s1 * ab3;
+            zb[1 + N1 + t] = fma(R(3) * s2 * z1, ab3, zb[1 + N1 + t]);
+            zb[1 + t] = fma(R(3) * fma(s3, z1s, s2 * z2), ab3, zb[1 + t]);
+            zb0 = fma(fma(s4 * z1s, z1, fma(R(3) * s3 * z1, z2, s2 * z3)), ab3, zb0);
+            a[1 + N1 + N2 + t] = fma(s3 * z1s, z1, fma(R(3) * s2 * z1, z2, s1 * z3));
         }
     }
     zb[0] = zb0;

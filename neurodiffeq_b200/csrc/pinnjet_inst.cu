@@ -1,19 +1,31 @@
 // pinnjet_inst.cu -- one translation unit per jet-channel scheme: compiled with -DPJ_N1=.. -DPJ_N2=.. (see build.py).
 // PJ_N1 = PJ_N2 = -1 builds the scheme-independent K2b reduce.  PJ_F64=1 builds the double FFMA kernels of the scheme
 // (launch_k1_f64_*, launch_k2_f64_*, occupancy_f64_*) from the same source; the tensor-core kernels are float only.
+// PJ_N3 > 0 (pure third-order channels) builds FFMA kernels only: the tensor-core kernels carry jets up to order 2.
+#ifndef PJ_WL
+#define PJ_WL 0
+#endif
+#ifndef PJ_N3
+#define PJ_N3 0
+#endif
+#define PJ_TC_UNIT (!PJ_F64 && PJ_N3 == 0)
+
 #include "pinnjet_k1.cuh"
 #include "pinnjet_k2.cuh"
-#if !PJ_F64
+#if PJ_TC_UNIT
 #include "pinnjet_k1tc3.cuh"
 #include "pinnjet_k2tc2.cuh"
 #endif
 
-#ifndef PJ_WL
-#define PJ_WL 0
-#endif
 #define PJ_CAT4(a, b, c, d) a##b##_##c##_##d
+#define PJ_CAT5(a, b, c, d, e) a##b##_##c##_##d##_##e
 #define PJ_NAME4(prefix, n1, n2, wl) PJ_CAT4(prefix, n1, n2, wl)
+#define PJ_NAME5(prefix, n1, n2, wl, n3) PJ_CAT5(prefix, n1, n2, wl, n3)
+#if PJ_N3 > 0   // launch_k1_1_1_0_1: the third-order schemes carry n3 in their names; the others keep theirs
+#define PJ_NAME(prefix, n1, n2) PJ_NAME5(prefix, n1, n2, PJ_WL, PJ_N3)
+#else
 #define PJ_NAME(prefix, n1, n2) PJ_NAME4(prefix, n1, n2, PJ_WL)
+#endif
 #if PJ_F64
 #define PJ_PREFIX_K1 launch_k1_f64_
 #define PJ_PREFIX_K2 launch_k2_f64_
@@ -74,7 +86,7 @@ constexpr int kEsz = 4;
 // CTAs per SM the register allocation is tuned for (shared memory may allow fewer): 128-thread CTAs share an SM
 constexpr int kMinB1_128 = 3, kMinB2_128 = 2;
 #endif
-constexpr int kP = ffma_tile_points(1 + PJ_N1 + PJ_N2, kEsz);
+constexpr int kP = ffma_tile_points(1 + PJ_N1 + PJ_N2 + PJ_N3, kEsz);
 
 // The kernel instance a plan selects and its block size.  `ready`: result of raising the instance's dynamic
 // shared-memory limit, done once per instance.
@@ -90,26 +102,26 @@ static Variant<Args> variant(void (*kern)(Args), int threads) {
 }
 
 static Variant<K1A> k1_variant(const Plan& pl) {
-#if !PJ_F64
+#if PJ_TC_UNIT
     if (pl.tc) {
         static const auto v = variant(k1tc3_forward_kernel<PJ_N1, PJ_N2, PJ_WL>, K1T_THREADS);
         return v;
     }
 #endif
     if (pl.ntc1 == 128) {
-        static const auto v = variant(PJ_K1_KERNEL<128, kMinB1_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(128));
+        static const auto v = variant(PJ_K1_KERNEL<128, kMinB1_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3>, ffma_k1_threads(128));
         return v;
     }
     if (pl.Q1 == FFMA_Q_WIDE) {
-        static const auto v = variant(PJ_K1_KERNEL<256, 1, kP, FFMA_Q_WIDE, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(256));
+        static const auto v = variant(PJ_K1_KERNEL<256, 1, kP, FFMA_Q_WIDE, PJ_N1, PJ_N2, PJ_WL, PJ_N3>, ffma_k1_threads(256));
         return v;
     }
-    static const auto v = variant(PJ_K1_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL>, ffma_k1_threads(256));
+    static const auto v = variant(PJ_K1_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3>, ffma_k1_threads(256));
     return v;
 }
 
 static Variant<K2A> k2_variant(const Plan& pl) {
-#if !PJ_F64
+#if PJ_TC_UNIT
     if (pl.tc) {
         static const auto v = variant(k2tc2_backward_kernel<PJ_N1, PJ_N2, PJ_WL>, K2T_THREADS);
         return v;
@@ -117,17 +129,17 @@ static Variant<K2A> k2_variant(const Plan& pl) {
 #endif
     if (pl.n_out_max > K2_OUT_GROUP) {
         if (pl.ntc == 128) {
-            static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, true>, ffma_k2_threads(128));
+            static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, true>, ffma_k2_threads(128));
             return v;
         }
-        static const auto v = variant(PJ_K2_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, true>, ffma_k2_threads(256));
+        static const auto v = variant(PJ_K2_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, true>, ffma_k2_threads(256));
         return v;
     }
     if (pl.ntc == 128) {
-        static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, false>, ffma_k2_threads(128));
+        static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, false>, ffma_k2_threads(128));
         return v;
     }
-    static const auto v = variant(PJ_K2_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, false>, ffma_k2_threads(256));
+    static const auto v = variant(PJ_K2_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, false>, ffma_k2_threads(256));
     return v;
 }
 

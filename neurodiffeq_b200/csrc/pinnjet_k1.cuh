@@ -71,10 +71,10 @@ struct RingCursor {
 
 // z-jets of P points of one unit (registers) -> workspace record (train), activation-jet rule, a-jets -> shared memory.
 // Record channel 0 holds tanh(z0) for tanh nets (the reverse pass then needs no transcendental) and z0 for sin nets.
-template <int P, int N1, int N2, int WL, typename R>
-__device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2], int act_kind, R* __restrict__ act_row, int T,
+template <int P, int N1, int N2, int WL, int N3, typename R>
+__device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2 + N3], int act_kind, R* __restrict__ act_row, int T,
                                             R* __restrict__ rec_row, int T2, const R (&wq)[P][WL > 0 ? WL : 1]) {
-    constexpr int C = 1 + N1 + N2;
+    constexpr int C = 1 + N1 + N2 + N3;
     auto store = [](R* dst, const R (&v)[P][C], int c) {
         if constexpr (P == 4)
             store4(dst, v[0][c], v[1][c], v[2][c], v[3][c]);
@@ -89,7 +89,7 @@ __device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2], int act_kin
         for (int c = 1; c < C; ++c) store(rec_row + c * T2, zq, c);
     }
 #pragma unroll
-    for (int p = 0; p < P; ++p) act_forward<N1, N2, WL>(act_kind, zq[p], wq[p]);
+    for (int p = 0; p < P; ++p) act_forward<N1, N2, WL, N3>(act_kind, zq[p], wq[p]);
     if (rec_row) {
         if (act_kind == PJ_ACT_TANH) {
 #pragma unroll
@@ -104,10 +104,10 @@ __device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2], int act_kin
     for (int c = 0; c < C; ++c) store(act_row + c * T, zq, c);
 }
 
-template <typename R, int NTC, int P, int Q, int N1, int N2, int WL>
+template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3>
 __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
     typedef typename Pair<R>::type pair;
-    constexpr int C = 1 + N1 + N2;
+    constexpr int C = 1 + N1 + N2 + N3;
     // service warps after the compute warps: 128-thread CTAs (weights always resident: the producer only issues the initial
     // loads) use ONE warp as producer-then-program warp; 256-thread CTAs have a producer warp and a program warp
     constexpr int N_SVC = NTC == 128 ? 1 : 2;
@@ -282,9 +282,9 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
 #pragma unroll
                             for (int f = 0; f < N1; ++f) zq[p][1 + f] = dz[f];
 #pragma unroll
-                            for (int s2 = 0; s2 < N2; ++s2) zq[p][1 + N1 + s2] = 0.0f;
+                            for (int s2 = 0; s2 < N2 + N3; ++s2) zq[p][1 + N1 + s2] = 0.0f;   // second and third orders: 0
                         }
-                        finish_unit<P, N1, N2, WL>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
+                        finish_unit<P, N1, N2, WL, N3>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
                     }
                 }
             }
@@ -323,7 +323,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
                         for (int c = 0; c < C; ++c)
 #pragma unroll
                             for (int p = 0; p < P; ++p) zq[p][c] = pick<P>(acc[q][c], p) + (c == 0 ? bias : 0.0f);
-                        finish_unit<P, N1, N2, WL>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
+                        finish_unit<P, N1, N2, WL, N3>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
                     }
                 }
                 bar_compute<NTC>();
@@ -366,13 +366,13 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
 }
 
 // The float and double kernels: one body (element type R); the float instance keeps its name and argument type.
-template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL>
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3>
 __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(const __grid_constant__ K1Args A) {
-    k1_forward_body<float, NTC, P, Q, N1, N2, WL>(A);
+    k1_forward_body<float, NTC, P, Q, N1, N2, WL, N3>(A);
 }
-template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL>
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3>
 __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel_f64(const __grid_constant__ K1ArgsF64 A) {
-    k1_forward_body<double, NTC, P, Q, N1, N2, WL>(A);
+    k1_forward_body<double, NTC, P, Q, N1, N2, WL, N3>(A);
 }
 
 }  // namespace pj

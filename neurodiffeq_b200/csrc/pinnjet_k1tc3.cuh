@@ -350,7 +350,7 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
                     a[c] = z[c][k];
                     rec[c][k] = z[c][k];
                 }
-                act_forward<N1, N2, WL>(act_kind, a, wq);
+                act_forward<N1, N2, WL, 0>(act_kind, a, wq);
                 if (act_kind == PJ_ACT_TANH) rec[0][k] = a[0];
 #pragma unroll
                 for (int c = 0; c < C; ++c) z[c][k] = a[c];

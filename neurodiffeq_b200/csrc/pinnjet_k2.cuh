@@ -41,10 +41,10 @@ __device__ __forceinline__ void wgrad_tile(typename Pair<R>::type (&acc)[WJ][WK]
 }
 
 // WIDE: some net has more than K2_OUT_GROUP outputs (a separate instance: the <= 4-output code stays as it is)
-template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, bool WIDE>
+template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
 __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     typedef typename Pair<R>::type pair;
-    constexpr int C = 1 + N1 + N2;
+    constexpr int C = 1 + N1 + N2 + N3;
     constexpr int NT_COMPUTE = NTC, NT_TOTAL = NTC + 32, N_CWARPS = NTC / 32;
     extern __shared__ __align__(128) unsigned char smem[];
     const PjSpec& sp = A.spec;
@@ -162,7 +162,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
 #pragma unroll
                                     for (int c = 0; c < C; ++c) ab[c] = fma(w, ybar[(o * C + c) * T + pt], ab[c]);
                                 }
-                            act_backward<N1, N2, WL>(act_kind, z, ab, a, zb, wq[p]);
+                            act_backward<N1, N2, WL, N3>(act_kind, z, ab, a, zb, wq[p]);
 #pragma unroll
                             for (int o = 0; o < K2_OUT_GROUP; ++o)
                                 if (o < n_out) {
@@ -216,7 +216,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
 #pragma unroll
                                 for (int c = 0; c < C; ++c) ab[c] = fma(w, ybar[(o * C + c) * T + pt], ab[c]);
                             }
-                            act_backward<N1, N2, WL>(act_kind, z, ab, a, zb, wq[p]);
+                            act_backward<N1, N2, WL, N3>(act_kind, z, ab, a, zb, wq[p]);
                             gb += zb[0];
 #pragma unroll
                             for (int c = 0; c < C; ++c) {
@@ -320,7 +320,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                                 z[c] = Zb[u * RS + c * T + p0 + p];
                                 ab[c] = pick<P>(acc[q][c], p);
                             }
-                            act_backward<N1, N2, WL>(act_kind, z, ab, av[p], zv[p], wq[p]);
+                            act_backward<N1, N2, WL, N3>(act_kind, z, ab, av[p], zv[p], wq[p]);
                             gb += zv[p][0];
                         }
 #pragma unroll
@@ -456,13 +456,13 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
 }
 
 // The float and double kernels: one body (element type R); the float instance keeps its name and argument type.
-template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, bool WIDE>
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
 __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
-    k2_backward_body<float, NTC, P, Q, N1, N2, WL, WIDE>(A);
+    k2_backward_body<float, NTC, P, Q, N1, N2, WL, N3, WIDE>(A);
 }
-template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, bool WIDE>
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
 __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel_f64(const __grid_constant__ K2ArgsF64 A) {
-    k2_backward_body<double, NTC, P, Q, N1, N2, WL, WIDE>(A);
+    k2_backward_body<double, NTC, P, Q, N1, N2, WL, N3, WIDE>(A);
 }
 
 }  // namespace pj

@@ -279,7 +279,7 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
 #pragma unroll
                             for (int c = 0; c < C; ++c) ab[c] = fmaf(w, yb_[o][c], ab[c]);
                         }
-                    act_backward<N1, N2, WL>(act_kind, z, ab, a, zbk, wq);
+                    act_backward<N1, N2, WL, 0>(act_kind, z, ab, a, zbk, wq);
 #pragma unroll
                     for (int c = 0; c < C; ++c) zb[c][k] = zbk[c];
                     gbv[k] = zbk[0];
@@ -367,7 +367,7 @@ __global__ void __launch_bounds__(K2T_THREADS, 1) k2tc2_backward_kernel(const __
                         z[c] = zr[c][k];
                         abk[c] = ab[c][k];
                     }
-                    act_backward<N1, N2, WL>(act_kind, z, abk, a, zbk, wq);
+                    act_backward<N1, N2, WL, 0>(act_kind, z, abk, a, zbk, wq);
 #pragma unroll
                     for (int c = 0; c < C; ++c) zb[c][k] = zbk[c];
                     gbv[k] = zbk[0];

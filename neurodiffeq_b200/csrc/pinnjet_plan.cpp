@@ -148,7 +148,10 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     if (prog_len > PROG_MAX) return fail(-2, "residual program too long (%d > %d instructions)", prog_len, PROG_MAX);
     if (sp.n_slots < 1 || sp.n_slots > SLOTS_MAX) return fail(-2, "n_slots=%d out of range (1..%d)", sp.n_slots, SLOTS_MAX);
     if (sp.wl < 0 || sp.wl > sp.n1 || (sp.wl > 0 && sp.n2 != 1)) return fail(-1, "inconsistent wl=%d (n1=%d, n2=%d)", sp.wl, sp.n1, sp.n2);
-    const int C = 1 + sp.n1 + sp.n2;
+    // a third-order channel needs the first and second channel of its direction; the combined channel has no pure seconds
+    if (sp.n3 < 0 || sp.n3 > sp.n2 || (sp.n3 > 0 && sp.wl != 0))
+        return fail(-1, "inconsistent n3=%d (n2=%d, wl=%d)", sp.n3, sp.n2, sp.wl);
+    const int C = 1 + sp.n1 + sp.n2 + sp.n3;
     pl.C = C;
     pl.P = ffma_tile_points(C, esz);
     pl.Q = FFMA_Q;
@@ -237,10 +240,10 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
 
     // ---- kernel selection ----
     // Tensor-core kernels (pinnjet_tc.cuh): every hidden layer exactly 64 wide (after padding), at most 8 jet channels, at
-    // most 4 outputs per net (one 16-byte row of the output Linear), the weight images of both kernels resident in shared
-    // memory.  The decision may not depend on the program length (only
+    // most 4 outputs per net (one 16-byte row of the output Linear), no third-order channels, the weight images of both
+    // kernels resident in shared memory.  The decision may not depend on the program length (only
     // pj_forward* know it): the programs get a fixed reserve.
-    bool tc = esz == 4 && dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4;
+    bool tc = esz == 4 && dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4 && sp.n3 == 0;
     for (int n = 0; tc && n < sp.n_nets; ++n)
         for (int h = 1; h < sp.net[n].n_linear; ++h) tc = tc && pl.hp[n][h] == TC_H;
     if (tc) {   // both kernels tile like the forward kernel; seeds / weights / records are shared as is

@@ -2,7 +2,8 @@
 nets / conditions / losses").
 
 The fused engine traces the user's callables once and runs them as jets inside two kernels; a problem it cannot express --
-derivatives of a network output beyond order 2 (nested operators, ``h1`` on a second-order PDE), more than four jet
+derivatives of a network output beyond order 2 (nested operators, ``h1`` on a second-order PDE; with ``jet_order=3`` only
+mixed third partials and fourth orders), more than four jet
 directions (full 3-D Hessians), activations without a jet rule (``Swish``, ``APTx``), modules that are not
 Linear/activation stacks (``MonomialNN``), data-dependent Python control flow, more networks / layers than the ABI holds --
 raises ``NotImplementedError`` / ``TypeError`` at construction.  The solvers then build an :class:`EagerProblem` instead,
@@ -209,13 +210,15 @@ _WARNED = set()
 
 
 def build_problem(fused_cls, nets, conditions, diff_eqs, n_coords, coords_for_condition=None, device=None, aux_outputs=None,
-                  enforce=None, **dtype):
+                  enforce=None, jet_order=None, **dtype):
     """``fused_cls(...)``, or -- when the tracer / planner refuses the problem -- an :class:`EagerProblem` with one warning per
     distinct reason.  Errors that are not refusals (no CUDA device, missing library, inconsistent shapes) propagate.
-    ``dtype=...``, when given, reaches both (``torch.float64``: the double kernels, or the autograd path in float64)."""
+    ``dtype=...``, when given, reaches both (``torch.float64``: the double kernels, or the autograd path in float64).
+    ``jet_order=...``, when given, reaches the fused class only (autograd differentiates to any order)."""
+    jet_kw = {} if jet_order is None else {"jet_order": jet_order}
     try:
         return fused_cls(nets, conditions, diff_eqs, n_coords, coords_for_condition=coords_for_condition, device=device,
-                         aux_outputs=aux_outputs, enforce=enforce, **dtype)
+                         aux_outputs=aux_outputs, enforce=enforce, **jet_kw, **dtype)
     except (NotImplementedError, TypeError) as exc:
         reason = f"{type(exc).__name__}: {exc}"
     if reason not in _WARNED:

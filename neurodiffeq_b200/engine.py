@@ -11,7 +11,7 @@ import numpy as np
 import torch
 
 from . import symbolic as S
-from .tracing import TracedProblem
+from .tracing import TracedProblem, check_jet_order
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("PINNJET_LIB", os.path.join(_HERE, "csrc", "libpinnjet.so"))
@@ -20,6 +20,7 @@ PJ_MAX_NETS, PJ_MAX_LINEAR, PJ_MAX_COORDS, PJ_MAX_DIRS = 4, 8, 8, 4
 SUPPORTED_SCHEMES = [(1, 0), (1, 1), (2, 0), (2, 1), (2, 2), (3, 0), (3, 3), (4, 4)]
 COMBINED_SCHEMES = [(2, 2), (3, 3), (4, 4)]   # (n1, n2) that also exist with ONE weighted second-order channel (wl = n2)
 COMBINED_ONLY = [(4, 4)]                      # ... and these exist ONLY in that form (9 separate channels do not fit)
+THIRD_ORDER_SCHEMES = [(1, 1, 1), (2, 1, 1)]  # (n1, n2, n3) with pure third-order channels (jet_order=3)
 
 
 def combine_seconds(n1, n2):
@@ -38,7 +39,8 @@ class PjSpec(ctypes.Structure):
                 ("n1", ctypes.c_int32), ("n2", ctypes.c_int32), ("wl", ctypes.c_int32),
                 ("dir", (ctypes.c_float * PJ_MAX_COORDS) * PJ_MAX_DIRS),
                 ("n_funcs", ctypes.c_int32), ("n_eq", ctypes.c_int32), ("n_yrows", ctypes.c_int32),
-                ("n_slots", ctypes.c_int32), ("n_theta", ctypes.c_int64), ("net", PjNet * PJ_MAX_NETS)]
+                ("n_slots", ctypes.c_int32), ("n_theta", ctypes.c_int64), ("net", PjNet * PJ_MAX_NETS),
+                ("n3", ctypes.c_int32)]
 
 
 class PjSizes(ctypes.Structure):
@@ -128,8 +130,14 @@ def _check(rc, what):
         raise RuntimeError(f"{what} failed ({rc}): {load_library().pj_last_error().decode()}")
 
 
-def pad_scheme(n1, n2):
-    """Smallest compiled channel scheme that covers (n1, n2)."""
+def pad_scheme(n1, n2, n3=0):
+    """Smallest compiled channel scheme that covers (n1, n2), or (n1, n2, n3) when there are third-order channels."""
+    if n3:
+        fits = [s for s in THIRD_ORDER_SCHEMES if s[0] >= n1 and s[1] >= n2 and s[2] >= n3]
+        if not fits:
+            raise NotImplementedError(f"no compiled kernel for jet channels (n1={n1}, n2={n2}, n3={n3}); "
+                                      f"available with third-order channels: {THIRD_ORDER_SCHEMES}")
+        return min(fits, key=sum)
     best = None
     for a, b in SUPPORTED_SCHEMES:
         if a >= n1 and b >= n2 and (best is None or (a + b) < sum(best)):
@@ -181,12 +189,15 @@ class FusedProblem:
     """Device state for one (nets, conditions, diff_eqs): spec, programs, flat parameter/gradient storage, workspace.
 
     ``dtype=torch.float64`` runs the problem on the double kernels (the ``_f64`` entry points): parameters, gradients,
-    coordinates, outputs and the loss are float64, the networks are converted to float64."""
+    coordinates, outputs and the loss are float64, the networks are converted to float64.
+    ``jet_order=3`` also runs residuals with pure third derivatives of a network output (``u'''``, ``u_xxx``) on the FFMA
+    kernels; problems without one trace exactly as with the default ``jet_order=2``."""
 
     dtype, f64, esz = torch.float32, False, 4   # set per instance by __init__
 
     def __init__(self, nets, conditions, diff_eqs, n_coords, coords_for_condition=None, device=None, aux_outputs=None,
-                 enforce=None, dtype=None):
+                 enforce=None, dtype=None, jet_order=2):
+        jet_order = check_jet_order(jet_order)
         self.lib = load_library()
         self.dtype = check_dtype(dtype)
         self.f64 = self.dtype == torch.float64
@@ -197,7 +208,8 @@ class FusedProblem:
             device = torch.device("cuda", torch.cuda.current_device())
         self.device = torch.device(device)
         self.tp = TracedProblem(nets, conditions, diff_eqs, n_coords, coords_for_condition, pad_scheme=pad_scheme,
-                                combine_seconds=combine_seconds, aux_outputs=aux_outputs, enforce=enforce)
+                                combine_seconds=combine_seconds, aux_outputs=aux_outputs, enforce=enforce,
+                                jet_order=jet_order)
         tp = self.tp
         if (tp.scheme.n1, tp.scheme.n2) in COMBINED_ONLY and not tp.wl:
             raise NotImplementedError(
@@ -306,6 +318,7 @@ class FusedProblem:
             raise NotImplementedError(f"{sp.n_nets} distinct networks (max {PJ_MAX_NETS})")
         sp.n1, sp.n2 = tp.scheme.n1, (1 if tp.wl else tp.scheme.n2)
         sp.wl = tp.wl
+        sp.n3 = tp.scheme.n3
         dirs = tp.direction_matrix()
         for f in range(tp.scheme.n1):
             for i in range(tp.n_coords):
@@ -368,7 +381,7 @@ class FusedProblem:
     def _accumulate_shortcut_grads(self, all_coords, n):
         """dL/dW_s of every Resnet instance from the seeds K1 left in the workspace: the raw output is (network jet +
         shortcut jet), so the seeds dL/d(jet) serve both; d(value)/dW_s[o][i] = x_i, d(first-order channel f)/dW_s[o][i]
-        = dir_f[i], second-order channels do not depend on W_s."""
+        = dir_f[i], second- and third-order channels do not depend on W_s."""
         info = self._plan_cache.get(n)
         if info is None:
             info = self._plan_cache[n] = self.plan_info(n)

@@ -26,7 +26,7 @@ import torch
 import torch.nn as nn
 
 from .conditions import BaseCondition
-from .engine import FusedProblem, check_dtype
+from .engine import FusedProblem, check_dtype, check_jet_order
 from .eager import build_problem
 from ._compat import renamed_arguments
 from .losses import _losses, h1_rows, h1_semi_rows
@@ -116,7 +116,11 @@ class BaseSolver:
 
     ``dtype``: ``None`` or ``torch.float32`` (the default) trains in float32; ``torch.float64`` -- the reference's precision
     -- converts the networks to float64 and runs the double kernels (or the autograd path in float64 for what the fused
-    engine refuses).  The device loop, ``optim.FlatAdam`` and the specialised kernel stay float32 only."""
+    engine refuses).  The device loop, ``optim.FlatAdam`` and the specialised kernel stay float32 only.
+
+    ``jet_order``: ``2`` (the default) runs derivatives of network outputs up to order 2 on the kernels and sends a problem
+    with a third derivative to the autograd path; ``3`` also runs pure third derivatives (``u'''``, ``u_xxx``, the ``h1``
+    loss on a 1-D second-order problem) on the FFMA kernels.  Mixed third partials and fourth orders fall back either way."""
 
     N_COORDS = None  # set by subclasses that know it a priori
 
@@ -124,9 +128,11 @@ class BaseSolver:
     def __init__(self, diff_eqs, conditions, nets=None, train_generator=None, valid_generator=None,
                  analytic_solutions=None, optimizer=None, loss_fn=None, n_batches_train=1, n_batches_valid=4,
                  metrics=None, n_input_units=None, n_output_units=None, shuffle=None, batch_size=None,
-                 device=None, data_parallel=True, device_loop=False, jit=None, dtype=None):
+                 device=None, data_parallel=True, device_loop=False, jit=None, dtype=None, jet_order=2):
         self.dtype = check_dtype(dtype)
-        dtype_kw = {"dtype": torch.float64} if self.dtype == torch.float64 else {}   # the float32 path is called as before
+        engine_kw = {"dtype": torch.float64} if self.dtype == torch.float64 else {}   # the float32 path is called as before
+        if check_jet_order(jet_order) == 3:   # ... and so is the order-2 path
+            engine_kw["jet_order"] = 3
         if shuffle:
             warnings.warn("param `shuffle` is deprecated and ignored; shuffling should be performed by generators",
                           FutureWarning)
@@ -175,7 +181,7 @@ class BaseSolver:
             self.problem = build_problem(FusedProblem, self.nets, self.conditions,
                                          h1_semi_rows(self._traced_diff_eqs, self.n_funcs),
                                          n_coords, coords_for_condition=self._coords_for_condition, device=device,
-                                         aux_outputs=self._traced_diff_eqs, enforce=self.compute_func_val, **dtype_kw)
+                                         aux_outputs=self._traced_diff_eqs, enforce=self.compute_func_val, **engine_kw)
             self.n_eq = len(self.problem.tp.aux_rows)
         else:
             # the fused engine (trace once -> kernels); what its tracer / planner refuses runs on the autograd path with one
@@ -183,7 +189,7 @@ class BaseSolver:
             self.problem = build_problem(FusedProblem, self.nets, self.conditions,
                                          self._h1_rows if self._h1 else self._traced_diff_eqs, n_coords,
                                          coords_for_condition=self._coords_for_condition, device=device,
-                                         enforce=self.compute_func_val, **dtype_kw)
+                                         enforce=self.compute_func_val, **engine_kw)
             self.n_eq = self.problem.n_eq - (n_coords if self._h1 else 0)     # the user's equations
         self.device = self.problem.device
         # The residual programs compiled INTO the forward kernel (jit.py: ~1 s of nvcc per problem, cached on disk; identical

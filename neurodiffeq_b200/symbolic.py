@@ -958,20 +958,23 @@ def substitute(roots, mapping):
 # jet channel scheme + lowering to bytecode
 # ----------------------------------------------------------------------------------------------------------------------
 class ChannelScheme:
-    """Which derivative channels the kernels carry: value, n1 first-order directional derivatives D_v, and the pure
-    second derivatives D_v D_v of the FIRST n2 directions.  Mixed partials are obtained by polarisation:
-    d2/dxi dxj = ( D_{ei+ej}^2 - D_ei^2 - D_ej^2 ) / 2, so pure directional seconds suffice for every order-2 jet."""
+    """Which derivative channels the kernels carry: value, n1 first-order directional derivatives D_v, the pure
+    second derivatives D_v D_v of the FIRST n2 directions and, with ``max_order=3``, the pure third derivatives D_v^3 of the
+    first n3 directions.  Mixed second partials are obtained by polarisation:
+    d2/dxi dxj = ( D_{ei+ej}^2 - D_ei^2 - D_ej^2 ) / 2, so pure directional seconds suffice for every order-2 jet.  Of order
+    3 only the pure partials d3/dxi3 exist (mixed ones would need third-order channels along polarisation directions)."""
 
-    def __init__(self, n_coords, multi_indices, merged=None):
+    def __init__(self, n_coords, multi_indices, merged=None, max_order=2):
         """``merged``: optional list of coordinate groups that may share ONE direction because no network instance takes
         two members of a group as inputs (constant coordinates of different boundary instances): the direction is the sum
-        of the group's axes, and restricted to any instance's inputs it is the axis of the one member that instance sees."""
+        of the group's axes, and restricted to any instance's inputs it is the axis of the one member that instance sees.
+        ``max_order``: 2, or 3 to accept pure third-order multi-indices ``(i, i, i)``."""
         self.n_coords = n_coords
         self._group = {}
         for grp in (merged or []):
             for i in grp:
                 self._group[i] = tuple(sorted(grp))
-        firsts, seconds = set(), set()
+        firsts, seconds, thirds = set(), set(), set()
         self.mixed = set()
         for alpha in multi_indices:
             if len(alpha) == 0:
@@ -989,17 +992,26 @@ class ChannelScheme:
                     seconds.add(self.axis(i))
                     seconds.add(self.axis(j))
                     seconds.add(self.mixed_dir(i, j))
+            elif len(alpha) == 3 and max_order >= 3:
+                if len(set(alpha)) != 1:
+                    raise NotImplementedError(
+                        f"mixed third-order derivative {tuple(alpha)} of a network output: the fused kernels carry pure "
+                        f"third-order jets only (d3/dx3 along one coordinate)")
+                thirds.add(self.axis(alpha[0]))
             else:
                 raise NotImplementedError(
                     f"derivative of order {len(alpha)} of a network output: the fused kernels carry jets up to "
-                    f"order 2 (SURVEY.md Appendix C caveat); higher orders are not implemented yet")
+                    f"order {min(max_order, 3)} (SURVEY.md Appendix C caveat); higher orders are not implemented yet")
+        seconds |= thirds
         firsts |= seconds
-        # directions with a second-order channel first, axis-aligned ones in coordinate order
+        # directions with a third-order channel first, then those with a second-order channel, then first-only ones;
+        # axis-aligned ones in coordinate order within each group
         key = lambda v: (sum(abs(x) for x in v) != 1.0, [-x for x in v])  # noqa: E731
-        sec_sorted = sorted(seconds, key=key)
+        third_sorted = sorted(thirds, key=key)
+        sec_sorted = third_sorted + sorted(seconds - thirds, key=key)
         first_only = sorted(firsts - seconds, key=key)
         self.dirs = sec_sorted + first_only
-        self.n1, self.n2 = len(self.dirs), len(sec_sorted)
+        self.n1, self.n2, self.n3 = len(self.dirs), len(sec_sorted), len(third_sorted)
 
     def axis(self, i):
         """direction vector that differentiates w.r.t. coordinate i (its whole group when directions are shared)"""
@@ -1012,16 +1024,17 @@ class ChannelScheme:
         """polarisation direction for d2/dxi dxj"""
         return tuple(a + b for a, b in zip(self.axis(i), self.axis(j)))
 
-    def pad_to(self, n1, n2):
-        """Add inert channels (zero direction vectors / unused second-order slots) up to a compiled (n1, n2)."""
-        if n1 < self.n1 or n2 < self.n2 or n2 > n1:
+    def pad_to(self, n1, n2, n3=0):
+        """Add inert channels (zero direction vectors / unused second- and third-order slots) up to a compiled
+        (n1, n2, n3)."""
+        if n1 < self.n1 or n2 < self.n2 or n3 < self.n3 or n2 > n1 or n3 > n2:
             raise ValueError("cannot shrink a channel scheme")
         self.dirs = list(self.dirs) + [tuple([0.0] * self.n_coords)] * (n1 - self.n1)
-        self.n1, self.n2 = n1, n2
+        self.n1, self.n2, self.n3 = n1, n2, n3
 
     @property
     def n_channels(self):
-        return 1 + self.n1 + self.n2
+        return 1 + self.n1 + self.n2 + self.n3
 
     def channel_of(self, alpha):
         """channel index of a (non-mixed) multi-index."""
@@ -1030,8 +1043,11 @@ class ChannelScheme:
         d = self.dirs.index(self.axis(alpha[0]))
         if len(alpha) == 1:
             return 1 + d
-        assert alpha[0] == alpha[1] and d < self.n2
-        return 1 + self.n1 + d
+        if len(alpha) == 2:
+            assert alpha[0] == alpha[1] and d < self.n2
+            return 1 + self.n1 + d
+        assert len(alpha) == 3 and len(set(alpha)) == 1 and d < self.n3
+        return 1 + self.n1 + self.n2 + d
 
     def second_channel_of_dir(self, v):
         d = self.dirs.index(tuple(v))

@@ -18,6 +18,15 @@ from .networks import SinActv
 ACT_TANH, ACT_SIN = 0, 1
 
 
+def check_jet_order(jet_order):
+    """``None`` / ``2`` (the default: jets up to order 2) or ``3`` (also pure third derivatives); else ``ValueError``."""
+    if jet_order is None or (isinstance(jet_order, int) and jet_order == 2):
+        return 2
+    if isinstance(jet_order, int) and jet_order == 3:
+        return 3
+    raise ValueError(f"jet_order must be 2 or 3, not {jet_order!r}")
+
+
 class NetDescription:
     """Static view of one distinct network: widths, activation, the nn.Linear modules, input coordinates."""
 
@@ -85,10 +94,12 @@ class NetDescription:
 
 class TracedProblem:
     def __init__(self, nets, conditions, diff_eqs, n_coords, coords_for_condition=None, pad_scheme=None,
-                 combine_seconds=None, aux_outputs=None, enforce=None):
+                 combine_seconds=None, aux_outputs=None, enforce=None, jet_order=2):
         """``nets[k]`` / ``conditions[k]`` as in the reference solver; ``diff_eqs(*funcs, *coords)``.
         ``coords_for_condition(k, cond, coords) -> tuple`` lets SolverSpherical trim coordinates
-        (reference solvers.py:894-916)."""
+        (reference solvers.py:894-916).  ``jet_order=3`` also accepts pure third derivatives of a network output
+        (``pad_scheme`` is then called with a third argument, n3, when the problem has any)."""
+        max_order = check_jet_order(jet_order)
         g = S.Graph()
         self.graph = g
         g.n_sampled = n_coords
@@ -140,9 +151,11 @@ class TracedProblem:
             if o >= self.nets[net_idx].n_out:
                 raise ValueError(f"condition selects output unit {o} of a network with "
                                  f"{self.nets[net_idx].n_out} outputs")
-        self.scheme = S.ChannelScheme(n_coords, [n.imm[2] for n in leaves], merged=self._mergeable_constant_coords())
+        self.scheme = S.ChannelScheme(n_coords, [n.imm[2] for n in leaves], merged=self._mergeable_constant_coords(),
+                                      max_order=max_order)
         if pad_scheme is not None:  # round the scheme up to one the engine has a compiled kernel for
-            self.scheme.pad_to(*pad_scheme(self.scheme.n1, self.scheme.n2))
+            sch = self.scheme
+            self.scheme.pad_to(*(pad_scheme(sch.n1, sch.n2, sch.n3) if sch.n3 else pad_scheme(sch.n1, sch.n2)))
         C = self.scheme.n_channels
         self.yrow0 = []
         row = 0
@@ -173,7 +186,8 @@ class TracedProblem:
         # C4: 7 -> 5); the executed FLOPs shrink accordingly, the result is the same function of theta.
         self.wl = 0
         self.weight_exprs = []
-        if combine_seconds is not None and combine_seconds(self.scheme.n1, self.scheme.n2):
+        # (not with third-order channels: their rule needs the pure seconds of their directions)
+        if combine_seconds is not None and not self.scheme.n3 and combine_seconds(self.scheme.n1, self.scheme.n2):
             self._try_combine_seconds()
             C = self.n_channels
             self.yrow0, row = [], 0

@@ -1,0 +1,54 @@
+"""ms/step of problems with a pure third derivative: y1 and t2 at 32768 points, t1 (KdV, 64 wide) at 16384, each on the
+third-order float kernels (``jet_order=3``), on the third-order double kernels, and on the autograd path in float32 (where
+these problems run with the default ``jet_order=2``) on the same GPU.  One step = pack + residual and parameter gradient of
+one batch (no optimizer), timed with CUDA events after a warm-up.  Prints one JSON line with the card's name and power limit.
+
+    python tools/bench_third_order.py [--steps 50] [--warmup 5]
+"""
+import argparse
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+import torch  # noqa: E402
+
+import workloads  # noqa: E402
+from bench_basis import _card, _ms_per_step  # noqa: E402
+
+CASES = (("y1", 32768), ("t2", 32768), ("t1", 16384))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=5)
+    args = ap.parse_args()
+    from neurodiffeq_b200.eager import EagerProblem
+    from neurodiffeq_b200.engine import FusedProblem
+    torch.cuda.set_device(0)
+    dev = torch.device("cuda", 0)
+    out = {"card": _card(), "steps": args.steps}
+    for key, n in CASES:
+        wl = workloads.build(workloads.product_namespace(), key)
+        coords = [torch.from_numpy(c).cuda() for c in workloads.sample_coords(wl, n, seed=1)]
+        args_of = lambda nets, conds: (nets, conds, workloads.bundle_eq_wrapper(wl), len(wl.coord_names),  # noqa: E731
+                                       workloads.coords_for_condition(key))
+        torch.manual_seed(0)
+        fp = FusedProblem(*args_of(wl.make_nets(), wl.make_conditions()), device=dev, jet_order=3)
+        out[f"{key}_n{n}_fp32_fused_ms"] = _ms_per_step(fp, coords, args.steps, args.warmup)
+        torch.manual_seed(0)
+        fp = FusedProblem(*args_of(wl.make_nets(), wl.make_conditions()), device=dev, jet_order=3, dtype=torch.float64)
+        out[f"{key}_n{n}_fp64_fused_ms"] = _ms_per_step(fp, coords, args.steps, args.warmup)
+        torch.manual_seed(0)
+        ep = EagerProblem(*args_of(wl.make_nets(), wl.make_conditions()), device=dev)
+        out[f"{key}_n{n}_fp32_autograd_ms"] = _ms_per_step(ep, coords, max(args.steps // 5, 5), 2)
+        out[f"{key}_fused_speedup"] = round(out[f"{key}_n{n}_fp32_autograd_ms"] / out[f"{key}_n{n}_fp32_fused_ms"], 1)
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()

@@ -271,6 +271,42 @@ def _biharmonic(nd):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# T1, T2  pure third derivatives of a network output: the fused kernels' third-order channels (jet_order=3)
+# ----------------------------------------------------------------------------------------------------------------------
+def _kdv(nd):
+    """Korteweg-de Vries  u_t + 6 u u_x + u_xxx = 0  on [-1, 1] x [0, 1] (IBVP1D, Dirichlet ends): channels (x, t) firsts,
+    x second and third; a 64-wide network, which the tensor-core kernels would otherwise take."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(64, 64))]
+
+    def make_conditions():
+        return [nd.IBVP1D(x_min=-1, x_max=1, t_min=0, t_min_val=lambda x: -torch.sin(np.pi * x),
+                          x_min_val=lambda t: 0, x_max_val=lambda t: 0)]
+
+    def diff_eqs(u, x, t):
+        return [nd.diff(u, t) + 6 * u * nd.diff(u, x) + nd.diff(u, x, order=3)]
+
+    return Workload("t1_kdv", "Solver2D", ("x", "t"), ((-1.0, 1.0), (0.0, 1.0)), [((2, 64, 64, 1), "tanh")], make_nets,
+                    make_conditions, diff_eqs, 1, 16384, _fcnn_flops((2, 64, 64, 1), 5), None)
+
+
+def _third_order_sin(nd):
+    """Blasius-type  u''' + u u'' / 2 = exp(-t),  u(0) = u'(0) = 0, with a SinActv network (the sine branch of the
+    fourth derivative in the reverse pass)."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(32, 32), actv=nd.SinActv)]
+
+    def make_conditions():
+        return [nd.IVP(t_0=0.0, u_0=0.0, u_0_prime=0.0)]
+
+    def diff_eqs(u, t):
+        return [nd.diff(u, t, order=3) + 0.5 * u * nd.diff(u, t, order=2) - torch.exp(-t)]
+
+    return Workload("t2_third_order_sin", "Solver1D", ("t",), ((0.0, 2.0),), [((1, 32, 32, 1), "sin")], make_nets,
+                    make_conditions, diff_eqs, 1, 32768, _fcnn_flops((1, 32, 32, 1), 4), None)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # S1..S3  networks with more than 4 outputs: spherical-harmonic expansions u = sum_k R_k(r) Y_k(theta, phi) of a network
 # that sees only r (reference function_basis.py, conditions.py:1023-1166), and a 6-output ODE system
 # ----------------------------------------------------------------------------------------------------------------------
@@ -369,6 +405,10 @@ _BUILDERS.update(_FALLBACK)
 _BASIS = {"s1": _s1, "s2": _s2, "s3": _s3}
 BASIS_NAMES = tuple(_BASIS)
 _BUILDERS.update(_BASIS)
+# pure third derivatives (jet_order=3); kept out of the tuples above as well
+_THIRD_ORDER = {"t1": _kdv, "t2": _third_order_sin}
+THIRD_ORDER_NAMES = tuple(_THIRD_ORDER)
+_BUILDERS.update(_THIRD_ORDER)
 # workloads whose conditions see only the first coordinate (a network of r alone, as SolverSpherical passes it)
 _RADIAL = ("s1", "s2")
 
