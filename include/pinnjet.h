@@ -36,7 +36,8 @@ extern "C" {
 #endif
 
 #define PJ_ABI_VERSION 2
-#define PJ_MAX_NETS 4
+#define PJ_MAX_NETS 4      /* network instances in PjSpec.net (the tensor-core kernels take at most this many)  */
+#define PJ_MAX_NETS_ALL 16 /* network instances per problem: net[0..3], then net_more[0..11] (FFMA kernels)  */
 #define PJ_MAX_OUT 32     /* output units per network (the tensor-core kernels take at most 4) */
 #define PJ_MAX_LINEAR 8   /* nn.Linear layers per network (hidden layers + 1) */
 #define PJ_MAX_COORDS 8
@@ -77,7 +78,13 @@ typedef struct PjSpec {
     int32_t n3;                         /* pure third-order channels of the first n3 directions, after the    */
                                         /* n2 channels (n3 <= n2, wl == 0); 0: none.  Appended last, so a     */
                                         /* zero-initialised spec of an older caller means what it meant       */
+    PjNet net_more[PJ_MAX_NETS_ALL - PJ_MAX_NETS];   /* instances 4..n_nets-1.  Read only when n_nets > 4, so a  */
+                                        /* caller whose struct ends at n3 keeps working with up to 4 nets     */
 } PjSpec;
+
+/* Network instance n (0 <= n < n_nets) of a spec: net[n], then net_more[n - PJ_MAX_NETS].  A macro, so that host code, device
+ * code and C callers share it (it evaluates n more than once). */
+#define PJ_SPEC_NET(spec, n) ((n) < PJ_MAX_NETS ? &(spec)->net[(n)] : &(spec)->net_more[(n) - PJ_MAX_NETS])
 
 /* Sizes the caller needs to allocate buffers (all bytes; workspace contents are opaque). */
 typedef struct PjSizes {
@@ -99,7 +106,9 @@ int pj_sizes(const PjSpec* spec, int64_t n_points, PjSizes* out);
  * out[0..18] = T,P,Q,C,RS,n_tiles,grid,hmax,n_stage_fwd,n_stage_bwd,resident_fwd,resident_bwd,zj_tile_floats,
  *              ws_zj,ws_seed,ws_gpart,ws_bytes,smem_fwd,smem_bwd; then hp[net][0..8] and zj_off[net][0..7] per net; then
  *              tc, tc_bwd (1: the forward and reverse kernels of this problem run on the tensor cores; always equal), tile points of those
- *              kernels, ws_tcrec, grid_bwd, n_tiles_fwd.  T / n_tiles describe the layout of the seeds in the workspace. */
+ *              kernels, ws_tcrec, grid_bwd, n_tiles_fwd; then hp / zj_off of nets 4..PJ_MAX_NETS_ALL-1 (the per-net block
+ *              above, appended so that the older layout stays a prefix).  T / n_tiles describe the layout of the seeds in the
+ *              workspace. */
 int pj_plan_info(const PjSpec* spec, int64_t n_points, int64_t* out, int32_t n_out);
 
 /* Re-layout the live parameters for the kernels (K-major + padded copies).  Call after every optimizer step.

@@ -1,5 +1,6 @@
 // pinnjet_api.cu -- C ABI of libpinnjet.so (include/pinnjet.h): the planner on the current device, the pack kernel and the
 // launch wrappers.
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <cstdarg>
@@ -77,6 +78,15 @@ static int fail(int code, const char* fmt, ...) {
     return code;
 }
 
+// The caller's spec as a kernel argument.  A caller built against a header whose PjSpec ends at n3 passes a shorter struct:
+// net_more is read only when the spec says it is there (n_nets > PJ_MAX_NETS), and is zero in the copy otherwise.
+static void copy_spec(PjSpec& dst, const PjSpec& src) {
+    const size_t head = offsetof(PjSpec, net_more);
+    const bool more = src.n_nets > PJ_MAX_NETS;
+    memcpy(&dst, &src, more ? sizeof(PjSpec) : head);
+    if (!more) memset(reinterpret_cast<char*>(&dst) + head, 0, sizeof(PjSpec) - head);
+}
+
 static const SchemeEntry* find_scheme(const PjSpec& sp) {
     for (const auto& e : kSchemes)
         if (e.n1 == sp.n1 && e.n2 == sp.n2 && e.wl == sp.wl && e.n3 == sp.n3) return &e;
@@ -150,7 +160,7 @@ __global__ void pack_kernel(const __grid_constant__ PackArgs A, const R* __restr
     }
     const int n = blockIdx.x / PJ_MAX_LINEAR, l = blockIdx.x % PJ_MAX_LINEAR;
     if (n >= sp.n_nets) return;
-    const PjNet& net = sp.net[n];
+    const PjNet& net = *PJ_SPEC_NET(&sp, n);
     const int L = net.n_linear - 1;
     if (l > L) return;
     const int fin = net.width[l], fout = net.width[l + 1];
@@ -254,12 +264,14 @@ static int plan_info_impl(const PjSpec* spec, int64_t n_points, int64_t* out, in
                                 pl.ws_bytes, pl.k1_bytes, pl.k2_bytes};
     int k = 0;
     for (int i = 0; i < 19 && k < n_out; ++i) out[k++] = head[i];
-    for (int n = 0; n < PJ_MAX_NETS; ++n) {
+    auto per_net = [&](int n) {
         for (int l = 0; l <= PJ_MAX_LINEAR && k < n_out; ++l) out[k++] = pl.hp[n][l];
         for (int l = 0; l < PJ_MAX_LINEAR && k < n_out; ++l) out[k++] = pl.zj_off[n][l];
-    }
+    };
+    for (int n = 0; n < PJ_MAX_NETS; ++n) per_net(n);
     const long long tail[6] = {pl.tc, pl.tc /* tc_bwd: the reverse kernel always matches the forward kernel */, pl.tp, pl.ws_tcrec, pl.grid_bwd, pl.n_tiles1};
     for (int i = 0; i < 6 && k < n_out; ++i) out[k++] = tail[i];
+    for (int n = PJ_MAX_NETS; n < PJ_MAX_NETS_ALL; ++n) per_net(n);   // nets 4..15, after the older layout
     return 0;
 }
 
@@ -267,7 +279,7 @@ template <typename R>
 static int pack_impl(const PjSpec* spec, const R* theta, R* theta_pack, R* zero_buf, long long n_zero, void* stream) {
     if (!spec || !theta || !theta_pack) return fail(-1, "null argument");
     PackArgs a;
-    a.spec = *spec;
+    copy_spec(a.spec, *spec);
     if (int rc = device_plan<R>(*spec, 1, 0, a.plan)) return rc;
     pack_kernel<R><<<dim3(spec->n_nets * PJ_MAX_LINEAR, PACK_PARTS), 256, 0, (cudaStream_t)stream>>>(a, theta, theta_pack, zero_buf, n_zero);
     return check_cuda(cudaGetLastError(), "pack launch");
@@ -332,7 +344,8 @@ static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, con
     if (!spec || !prog || !coords || !theta_pack || !ws) return fail(-1, "null argument");
     typename ArgsOf<R>::K1 a;
     memset(&a, 0, sizeof(a));
-    a.spec = *spec;
+    copy_spec(a.spec, *spec);
+    for (int n = 0; n < spec->n_nets && n < PJ_MAX_NETS_ALL; ++n) a.net[n] = *PJ_SPEC_NET(spec, n);
     if (spec->wl > 0 && (!prog_w || prog_w_len < 1)) return fail(-1, "spec->wl=%d needs a weight program", spec->wl);
     if (spec->wl == 0) prog_w_len = 0;
     if (int rc = device_plan<R>(*spec, n, prog_len, a.plan, prog_w_len)) return rc;
@@ -445,7 +458,8 @@ static int run_k2(const PjSpec* spec, const R* const* coords, int64_t n_points, 
     if (!spec || !coords || !theta_pack || !workspace) return fail(-1, "null argument");
     typename ArgsOf<R>::K2 a;
     memset(&a, 0, sizeof(a));
-    a.spec = *spec;
+    copy_spec(a.spec, *spec);
+    for (int n = 0; n < spec->n_nets && n < PJ_MAX_NETS_ALL; ++n) a.net[n] = *PJ_SPEC_NET(spec, n);
     if (int rc = device_plan<R>(*spec, n_points, 0, a.plan)) return rc;
     if (workspace_bytes < (size_t)a.plan.ws_bytes)
         return fail(-1, "workspace too small: %zu < %lld bytes", workspace_bytes, a.plan.ws_bytes);

@@ -60,6 +60,7 @@ template <typename R>
 struct K1ArgsT {
     PjSpec spec;
     Plan plan;
+    PjNet net[PJ_MAX_NETS_ALL];          // PJ_SPEC_NET(&spec, n) for n < spec.n_nets, contiguous: what the FFMA kernels index
     const R* coords[PJ_MAX_COORDS];
     const R* pack;
     const int4* prog;
@@ -85,6 +86,7 @@ template <typename R>
 struct K2ArgsT {
     PjSpec spec;
     Plan plan;
+    PjNet net[PJ_MAX_NETS_ALL];          // PJ_SPEC_NET(&spec, n) for n < spec.n_nets, contiguous: what the FFMA kernels index
     const R* coords[PJ_MAX_COORDS];
     const R* pack;
     long long N;

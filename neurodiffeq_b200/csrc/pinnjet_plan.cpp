@@ -11,16 +11,20 @@ namespace pj {
 static int round_up(int v, int m) { return (v + m - 1) / m * m; }
 static long long round_up_ll(long long v, long long m) { return (v + m - 1) / m * m; }
 
+static const PjNet& net_of(const PjSpec& sp, int n) { return *PJ_SPEC_NET(&sp, n); }   // instance n < sp.n_nets
+
 static int max_outputs(const PjSpec& sp) {   // widest output Linear of all nets
     int m = 0;
-    for (int i = 0; i < sp.n_nets; ++i)
-        if (sp.net[i].width[sp.net[i].n_linear] > m) m = sp.net[i].width[sp.net[i].n_linear];
+    for (int i = 0; i < sp.n_nets; ++i) {
+        const PjNet& net = net_of(sp, i);
+        if (net.width[net.n_linear] > m) m = net.width[net.n_linear];
+    }
     return m;
 }
 
 static int hidden_linears(const PjSpec& sp) {   // hidden->hidden Linears of all nets
     int n = 0;
-    for (int i = 0; i < sp.n_nets; ++i) n += sp.net[i].n_linear - 2;
+    for (int i = 0; i < sp.n_nets; ++i) n += net_of(sp, i).n_linear - 2;
     return n;
 }
 
@@ -142,7 +146,8 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
                         Plan& pl, int* occ_min, const Err& fail, int esz) {
     memset(&pl, 0, sizeof(pl));
     if (sp.abi_version != PJ_ABI_VERSION) return fail(-1, "PjSpec.abi_version %d != %d", sp.abi_version, PJ_ABI_VERSION);
-    if (sp.n_nets < 1 || sp.n_nets > PJ_MAX_NETS) return fail(-1, "n_nets=%d out of range", sp.n_nets);
+    if (sp.n_nets < 1 || sp.n_nets > PJ_MAX_NETS_ALL)
+        return fail(-1, "n_nets=%d out of range (1..%d)", sp.n_nets, PJ_MAX_NETS_ALL);
     if (sp.n_coords < 1 || sp.n_coords > PJ_MAX_COORDS) return fail(-1, "n_coords=%d out of range", sp.n_coords);
     if (N < 1) return fail(-1, "n_points must be positive");
     if (prog_len > PROG_MAX) return fail(-2, "residual program too long (%d > %d instructions)", prog_len, PROG_MAX);
@@ -157,7 +162,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     pl.Q = FFMA_Q;
     int hmax = 32, yrows = 0;
     for (int n = 0; n < sp.n_nets; ++n) {
-        const PjNet& net = sp.net[n];
+        const PjNet& net = net_of(sp, n);
         if (net.n_linear < 2 || net.n_linear > PJ_MAX_LINEAR) return fail(-1, "net %d: n_linear=%d out of range", n, net.n_linear);
         if (net.n_in < 1 || net.n_in > PJ_MAX_COORDS || net.width[0] != net.n_in) return fail(-1, "net %d: bad n_in", n);
         const int n_out = net.width[net.n_linear];
@@ -196,7 +201,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     // ---- packed parameters ----
     int off = 0;
     for (int n = 0; n < sp.n_nets; ++n) {
-        const PjNet& net = sp.net[n];
+        const PjNet& net = net_of(sp, n);
         const int L = net.n_linear - 1, n_out = net.width[net.n_linear];
         pl.s_wt0[n] = off; off += round_up(net.n_in * pl.hp[n][1], 4);
         pl.s_dz[n] = off; off += PJ_MAX_DIRS * pl.hp[n][1];
@@ -209,7 +214,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     long long big = off;
     pl.chunks_fwd = pl.chunks_bwd = 0;
     for (int n = 0; n < sp.n_nets; ++n) {
-        const int L = sp.net[n].n_linear - 1;
+        const int L = net_of(sp, n).n_linear - 1;
         for (int l = 1; l < L; ++l) {
             const int hi = pl.hp[n][l], ho = pl.hp[n][l + 1];
             pl.b_wt[n][l] = big; big += (long long)hi * ho;
@@ -228,7 +233,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     // ---- shared-memory gradient accumulators ----
     off = 0;
     for (int n = 0; n < sp.n_nets; ++n) {
-        const PjNet& net = sp.net[n];
+        const PjNet& net = net_of(sp, n);
         const int L = net.n_linear - 1, n_out = net.width[net.n_linear];
         pl.g_w0[n] = off; off += pl.hp[n][1] * net.n_in;
         for (int l = 0; l < L; ++l) { pl.g_b[n][l] = off; off += pl.hp[n][l + 1]; }
@@ -240,15 +245,16 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
 
     // ---- kernel selection ----
     // Tensor-core kernels (pinnjet_tc.cuh): every hidden layer exactly 64 wide (after padding), at most 8 jet channels, at
-    // most 4 outputs per net (one 16-byte row of the output Linear), no third-order channels, the weight images of both
-    // kernels resident in shared memory.  The decision may not depend on the program length (only
-    // pj_forward* know it): the programs get a fixed reserve.
-    bool tc = esz == 4 && dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4 && sp.n3 == 0;
+    // most 4 outputs per net (one 16-byte row of the output Linear), no third-order channels, at most PJ_MAX_NETS network
+    // instances (their register arrays are sized by it), the weight images of both kernels resident in shared memory.  The
+    // decision may not depend on the program length (only pj_forward* know it): the programs get a fixed reserve.
+    bool tc = esz == 4 && dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4 && sp.n3 == 0 &&
+              sp.n_nets <= PJ_MAX_NETS;
     for (int n = 0; tc && n < sp.n_nets; ++n)
-        for (int h = 1; h < sp.net[n].n_linear; ++h) tc = tc && pl.hp[n][h] == TC_H;
+        for (int h = 1; h < net_of(sp, n).n_linear; ++h) tc = tc && pl.hp[n][h] == TC_H;
     if (tc) {   // both kernels tile like the forward kernel; seeds / weights / records are shared as is
         int n_hidden = 0;
-        for (int n = 0; n < sp.n_nets; ++n) n_hidden += sp.net[n].n_linear - 1;
+        for (int n = 0; n < sp.n_nets; ++n) n_hidden += net_of(sp, n).n_linear - 1;
         Plan t = pl;
         t.tc = 1;
         t.tp = TC_ROWS / tc_channel_pad(C);
@@ -315,7 +321,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     // ---- workspace: loss partials | FFMA records | seeds | gradient partials | weights | tensor-core records ----
     long long zt = 0;
     for (int n = 0; n < sp.n_nets; ++n)
-        for (int h = 1; h < sp.net[n].n_linear; ++h) { pl.zj_off[n][h] = (int)zt; zt += (long long)pl.hp[n][h] * pl.RS; }
+        for (int h = 1; h < net_of(sp, n).n_linear; ++h) { pl.zj_off[n][h] = (int)zt; zt += (long long)pl.hp[n][h] * pl.RS; }
     pl.zj_tile_floats = zt;
     pl.ws_loss = 0;
     pl.ws_zj = LOSS_PART_BYTES;
@@ -335,9 +341,9 @@ int make_plan(const PjSpec& sp, long long N, int prog_len, int prog_w_len, const
     const Err fail{err, err_len};
     if (esz != 4 && esz != 8) return fail(-1, "element size %d (4 or 8)", esz);
     int occ = 0, hmax = 0;
-    for (int n = 0; n < sp.n_nets && n < PJ_MAX_NETS; ++n)
-        for (int h = 1; h < sp.net[n].n_linear && h <= PJ_MAX_LINEAR; ++h)
-            if (sp.net[n].width[h] > hmax) hmax = sp.net[n].width[h];
+    for (int n = 0; n < sp.n_nets && n < PJ_MAX_NETS_ALL; ++n)
+        for (int h = 1; h < net_of(sp, n).n_linear && h <= PJ_MAX_LINEAR; ++h)
+            if (net_of(sp, n).width[h] > hmax) hmax = net_of(sp, n).width[h];
     Plan narrow;
     int rc128 = -1;
     if (hmax <= 64) {

@@ -17,6 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("PINNJET_LIB", os.path.join(_HERE, "csrc", "libpinnjet.so"))
 
 PJ_MAX_NETS, PJ_MAX_LINEAR, PJ_MAX_COORDS, PJ_MAX_DIRS = 4, 8, 8, 4
+PJ_MAX_NETS_ALL = 16   # network instances per problem: PjSpec.net holds the first PJ_MAX_NETS, net_more the rest
 SUPPORTED_SCHEMES = [(1, 0), (1, 1), (2, 0), (2, 1), (2, 2), (3, 0), (3, 3), (4, 4)]
 COMBINED_SCHEMES = [(2, 2), (3, 3), (4, 4)]   # (n1, n2) that also exist with ONE weighted second-order channel (wl = n2)
 COMBINED_ONLY = [(4, 4)]                      # ... and these exist ONLY in that form (9 separate channels do not fit)
@@ -40,7 +41,11 @@ class PjSpec(ctypes.Structure):
                 ("dir", (ctypes.c_float * PJ_MAX_COORDS) * PJ_MAX_DIRS),
                 ("n_funcs", ctypes.c_int32), ("n_eq", ctypes.c_int32), ("n_yrows", ctypes.c_int32),
                 ("n_slots", ctypes.c_int32), ("n_theta", ctypes.c_int64), ("net", PjNet * PJ_MAX_NETS),
-                ("n3", ctypes.c_int32)]
+                ("n3", ctypes.c_int32), ("net_more", PjNet * (PJ_MAX_NETS_ALL - PJ_MAX_NETS))]
+
+    def net_at(self, n):
+        """network instance n: net[n] for the first PJ_MAX_NETS, then net_more (PJ_SPEC_NET of pinnjet.h)"""
+        return self.net[n] if n < PJ_MAX_NETS else self.net_more[n - PJ_MAX_NETS]
 
 
 class PjSizes(ctypes.Structure):
@@ -314,8 +319,8 @@ class FusedProblem:
         sp.abi_version = 2
         sp.n_coords = tp.n_coords
         sp.n_nets = len(tp.nets)
-        if sp.n_nets > PJ_MAX_NETS:
-            raise NotImplementedError(f"{sp.n_nets} distinct networks (max {PJ_MAX_NETS})")
+        if sp.n_nets > PJ_MAX_NETS_ALL:
+            raise NotImplementedError(f"{sp.n_nets} network instances (max {PJ_MAX_NETS_ALL})")
         sp.n1, sp.n2 = tp.scheme.n1, (1 if tp.wl else tp.scheme.n2)
         sp.wl = tp.wl
         sp.n3 = tp.scheme.n3
@@ -328,7 +333,7 @@ class FusedProblem:
                          ((tp.prog_w,) if tp.wl else ()))
         sp.n_theta = self.n_theta
         for n, nd in enumerate(tp.nets):
-            net = sp.net[n]
+            net = sp.net_at(n)
             net.n_in = nd.widths[0]
             for i, c in enumerate(nd.in_coord):
                 net.in_coord[i] = c
@@ -611,23 +616,30 @@ class FusedProblem:
         return ok
 
     def plan_info(self, n_points):
-        """Tiling plan (diagnostics): dict with T, RS, grid, ... plus padded widths and z-jet offsets per net."""
-        n = 19 + PJ_MAX_NETS * (2 * PJ_MAX_LINEAR + 1) + 6
+        """Tiling plan (diagnostics): dict with T, RS, grid, ... plus padded widths and z-jet offsets of all
+        PJ_MAX_NETS_ALL net slots (pj_plan_info: nets 0-3, six trailing fields, then nets 4-15)."""
+        per_net = 2 * PJ_MAX_LINEAR + 1
+        n = 19 + PJ_MAX_NETS * per_net + 6 + (PJ_MAX_NETS_ALL - PJ_MAX_NETS) * per_net
         out = (ctypes.c_int64 * n)()
         with torch.cuda.device(self.device):
             _check(self._fn("pj_plan_info")(ctypes.byref(self.spec), n_points, out, n), "pj_plan_info")
         keys = ("T P Q C RS n_tiles grid hmax n_stage_fwd n_stage_bwd resident_fwd resident_bwd zj_tile_floats ws_zj "
                 "ws_seed ws_gpart ws_bytes smem_fwd smem_bwd").split()
         info = {k: int(out[i]) for i, k in enumerate(keys)}
-        k = 19
         info["hp"], info["zj_off"] = [], []
-        for _ in range(PJ_MAX_NETS):
-            info["hp"].append([int(out[k + i]) for i in range(PJ_MAX_LINEAR + 1)])
-            k += PJ_MAX_LINEAR + 1
-            info["zj_off"].append([int(out[k + i]) for i in range(PJ_MAX_LINEAR)])
-            k += PJ_MAX_LINEAR
+
+        def nets(k, count):
+            for _ in range(count):
+                info["hp"].append([int(out[k + i]) for i in range(PJ_MAX_LINEAR + 1)])
+                k += PJ_MAX_LINEAR + 1
+                info["zj_off"].append([int(out[k + i]) for i in range(PJ_MAX_LINEAR)])
+                k += PJ_MAX_LINEAR
+            return k
+
+        k = nets(19, PJ_MAX_NETS)
         for i, name in enumerate(("tc", "tc_bwd", "tc_tile_points", "ws_tcrec", "grid_bwd", "n_tiles_fwd")):
             info[name] = int(out[k + i])
+        nets(k + 6, PJ_MAX_NETS_ALL - PJ_MAX_NETS)
         return info
 
     # ---- CUDA-graph replay of a whole residual+gradient evaluation -----------------------------------------------------

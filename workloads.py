@@ -382,6 +382,75 @@ def _s3(nd):
                     make_conditions, diff_eqs, K, 4096, _fcnn_flops((1, 32, 32, K), 2), None)
 
 
+# ----------------------------------------------------------------------------------------------------------------------
+# M1..M3  systems with more than 4 network instances: one network per function (the solvers' default), and Neumann ends
+# that evaluate each network again at a boundary abscissa
+# ----------------------------------------------------------------------------------------------------------------------
+def _m1(nd):
+    """SEIRD epidemic model: 5 compartments, one tanh network and one IVP per function (5 instances)."""
+    beta, sigma, gamma, mu = 1.2, 0.5, 0.25, 0.02
+    u0 = (0.97, 0.02, 0.01, 0.0, 0.0)
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(32, 32)) for _ in range(5)]
+
+    def make_conditions():
+        return [nd.IVP(t_0=0.0, u_0=v) for v in u0]
+
+    def diff_eqs(s, e, i, r, d, t):
+        return [nd.diff(s, t) + beta * s * i,
+                nd.diff(e, t) - beta * s * i + sigma * e,
+                nd.diff(i, t) - sigma * e + (gamma + mu) * i,
+                nd.diff(r, t) - gamma * i,
+                nd.diff(d, t) - mu * i]
+
+    return Workload("m1_seird", "Solver1D", ("t",), ((0.0, 10.0),), [((1, 32, 32, 1), "tanh")] * 5, make_nets,
+                    make_conditions, diff_eqs, 5, 32768, 5 * _fcnn_flops((1, 32, 32, 1), 2), None)
+
+
+def _m2(nd):
+    """Two-species reaction-diffusion in (x, t) with no-flux (Neumann) ends: one IBVP1D and one network per species, each
+    network evaluated in the interior and at both ends (6 instances)."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(64, 64)) for _ in range(2)]
+
+    def make_conditions():
+        return [nd.IBVP1D(x_min=0.0, x_max=1.0, t_min=0.0, t_min_val=lambda x: 0.5 + 0.25 * torch.cos(np.pi * x),
+                          x_min_prime=lambda t: 0.0 * t, x_max_prime=lambda t: 0.0 * t),
+                nd.IBVP1D(x_min=0.0, x_max=1.0, t_min=0.0, t_min_val=lambda x: 0.3 - 0.1 * torch.cos(np.pi * x),
+                          x_min_prime=lambda t: 0.0 * t, x_max_prime=lambda t: 0.0 * t)]
+
+    def diff_eqs(u, v, x, t):
+        return [nd.diff(u, t) - 0.1 * nd.diff(u, x, order=2) - u * (1 - u) + u * v,
+                nd.diff(v, t) - 0.05 * nd.diff(v, x, order=2) - 0.5 * u * v + 0.3 * v]
+
+    return Workload("m2_reaction_diffusion", "Solver2D", ("x", "t"), ((0.0, 1.0), (0.0, 1.0)),
+                    [((2, 64, 64, 1), "tanh")] * 2, make_nets, make_conditions, diff_eqs, 2, 16384,
+                    6 * _fcnn_flops((2, 64, 64, 1), 6), None)
+
+
+def _m3(nd):
+    """16-function linear chain u_i' = k (u_{i-1} - 2 u_i + u_{i+1}) with zero ends (method of lines for the heat equation):
+    16 networks alternating between 32-wide tanh and 64-wide SinActv (16 instances, mixed widths and activations)."""
+    K, k = 16, 2.0
+    shapes = [((1, 32, 32, 1), "tanh") if i % 2 == 0 else ((1, 64, 64, 1), "sin") for i in range(K)]
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(32, 32)) if i % 2 == 0 else
+                nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(64, 64), actv=nd.SinActv) for i in range(K)]
+
+    def make_conditions():
+        return [nd.IVP(t_0=0.0, u_0=math.sin(math.pi * (i + 1) / (K + 1))) for i in range(K)]
+
+    def diff_eqs(*args):
+        u, t = args[:K], args[K]
+        side = lambda j: u[j] if 0 <= j < K else 0.0   # noqa: E731
+        return [nd.diff(u[i], t) - k * (side(i - 1) - 2 * u[i] + side(i + 1)) for i in range(K)]
+
+    return Workload("m3_heat_chain", "Solver1D", ("t",), ((0.0, 1.0),), shapes, make_nets, make_conditions, diff_eqs, K,
+                    16384, sum(_fcnn_flops(w, 2) for w, _ in shapes), None)
+
+
 _EXTRA = {
     "x1": lambda nd: _heat(nd, "x1_heat_dirichlet_neumann", "right"),
     "x2": lambda nd: _heat(nd, "x2_heat_neumann_dirichlet", "left"),
@@ -409,6 +478,10 @@ _BUILDERS.update(_BASIS)
 _THIRD_ORDER = {"t1": _kdv, "t2": _third_order_sin}
 THIRD_ORDER_NAMES = tuple(_THIRD_ORDER)
 _BUILDERS.update(_THIRD_ORDER)
+# more than 4 network instances per problem; kept out of the tuples above as well
+_SYSTEM = {"m1": _m1, "m2": _m2, "m3": _m3}
+SYSTEM_NAMES = tuple(_SYSTEM)
+_BUILDERS.update(_SYSTEM)
 # workloads whose conditions see only the first coordinate (a network of r alone, as SolverSpherical passes it)
 _RADIAL = ("s1", "s2")
 
