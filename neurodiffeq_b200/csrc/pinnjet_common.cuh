@@ -475,12 +475,84 @@ __device__ __forceinline__ void gemm_rows(typename Pair<R>::type (&acc)[Q][C][P 
     }
 }
 
-// scalar view of a packed accumulator tile (p is a compile-time constant after unrolling)
+// The float adjoint GEMM of the reverse kernel: the same tile and the same FMA order per accumulator as gemm_rows, but
+// every point of the tile is a plain float register.  sm_90 has no packed FP32 FMA, and the 64-bit pairs only cost
+// register moves there (ptxas re-pairs the results at the loop back-edge).  The A and B operands of row k + 1 are loaded
+// before the FFMAs of row k, so the shared-memory latency hides behind them; the last row loads itself again instead of
+// reading past the chunk.
+template <int P, int Q, int C>
+__device__ __forceinline__ void gemm_rows(float (&acc)[Q][C][P], const float* __restrict__ a_ptr, int RS, int T,
+                                          const float* __restrict__ b_ptr, int ldb, int nrows) {
+    static_assert(Q % 4 == 0 && (P == 2 || P == 4), "float4 weight rows, float2 / float4 point rows");
+    auto load = [&](int k, float (&a)[C][P], float (&b)[Q]) {
+        const float* ar = a_ptr + k * RS;
+#pragma unroll
+        for (int c = 0; c < C; ++c) {
+            if constexpr (P == 4) {
+                const float4 v = *reinterpret_cast<const float4*>(ar + c * T);
+                a[c][0] = v.x;
+                a[c][1] = v.y;
+                a[c][2] = v.z;
+                a[c][3] = v.w;
+            } else {
+                const float2 v = *reinterpret_cast<const float2*>(ar + c * T);
+                a[c][0] = v.x;
+                a[c][1] = v.y;
+            }
+        }
+        const float* br = b_ptr + k * ldb;
+#pragma unroll
+        for (int q4 = 0; q4 < Q / 4; ++q4) {
+            const float4 v = *reinterpret_cast<const float4*>(br + 4 * q4);
+            b[4 * q4 + 0] = v.x;
+            b[4 * q4 + 1] = v.y;
+            b[4 * q4 + 2] = v.z;
+            b[4 * q4 + 3] = v.w;
+        }
+    };
+    if (nrows <= 0) return;
+    float a[C][P], b[Q];
+    load(0, a, b);
+#pragma unroll 2
+    for (int k = 0; k < nrows; ++k) {
+        float an[C][P], bn[Q];
+        load(min(k + 1, nrows - 1), an, bn);
+#pragma unroll
+        for (int q = 0; q < Q; ++q)
+#pragma unroll
+            for (int c = 0; c < C; ++c)
+#pragma unroll
+                for (int p = 0; p < P; ++p) acc[q][c][p] = fmaf(a[c][p], b[q], acc[q][c][p]);
+#pragma unroll
+        for (int c = 0; c < C; ++c)
+#pragma unroll
+            for (int p = 0; p < P; ++p) a[c][p] = an[c][p];
+#pragma unroll
+        for (int q = 0; q < Q; ++q) b[q] = bn[q];
+    }
+}
+
+// Accumulator tile of the reverse kernel's adjoint GEMM: plain floats (gemm_rows above) when SCALAR, point pairs for
+// double.
+template <typename R, int P, bool SCALAR>
+struct AdjAcc {
+    typedef typename Pair<R>::type elem;
+    static constexpr int n = P / 2;
+};
+template <int P>
+struct AdjAcc<float, P, true> {
+    typedef float elem;
+    static constexpr int n = P;
+};
+
+// scalar view of an accumulator tile (p is a compile-time constant after unrolling)
 template <int P, typename PairT>
 __device__ __forceinline__ auto pick(const PairT (&v)[P / 2], int p) {
     const auto t = unpack2(v[p >> 1]);
     return (p & 1) ? t.y : t.x;
 }
+template <int P>
+__device__ __forceinline__ float pick(const float (&v)[P], int p) { return v[p]; }
 
 // ---- optional phase timing (diagnostic build only: -DPJ_TIMING=1 -> libpinnjet_timing.so; never in the product) --------
 #ifdef PJ_TIMING

@@ -20,9 +20,10 @@ namespace pj {
 constexpr int WJ = 8, WK = 4;   // weight-gradient output tile per thread (8 rows of z_bar x 4 rows of a-jets)
 
 // out[j][k] += sum_r G[j][r] * Z[k][r],  r over the C*T (channel, point) pairs; rows interleaved over lanes so that the
-// 16-byte loads of 8 consecutive rows (stride RS = C*T + 16 bytes) hit 32 distinct banks.
+// 16-byte loads of 8 consecutive rows (stride RS = C*T + 16 bytes) hit 32 distinct banks.  Each output keeps two partial
+// sums (even and odd r for float, one pair of doubles), added in the epilogue (wgrad_sum).
 template <typename R>
-__device__ __forceinline__ void wgrad_tile(typename Pair<R>::type (&acc)[WJ][WK], const R* __restrict__ g_base, int j_step,
+__device__ __forceinline__ void wgrad_tile(typename Pair<R>::type (&acc)[WJ][WK][1], const R* __restrict__ g_base, int j_step,
                                            const R* __restrict__ z_base, int k_step, int RS, int n_r) {
     typedef typename Pair<R>::row16 row16;
     constexpr int STEP = 16 / sizeof(R);
@@ -36,15 +37,45 @@ __device__ __forceinline__ void wgrad_tile(typename Pair<R>::type (&acc)[WJ][WK]
 #pragma unroll
         for (int i = 0; i < WJ; ++i)
 #pragma unroll
-            for (int j = 0; j < WK; ++j) Pair<R>::fma16(acc[i][j], gv[i], zv[j]);
+            for (int j = 0; j < WK; ++j) Pair<R>::fma16(acc[i][j][0], gv[i], zv[j]);
     }
 }
+// float, the two partial sums as plain registers: the same FMAs in the same order as the pair form above, without the
+// register moves ptxas inserts to keep 64-bit pairs in place (sm_90 has no packed FP32 FMA)
+__device__ __forceinline__ void wgrad_tile(float (&acc)[WJ][WK][2], const float* __restrict__ g_base, int j_step,
+                                           const float* __restrict__ z_base, int k_step, int RS, int n_r) {
+#pragma unroll 2
+    for (int r = 0; r < n_r; r += 4) {
+        float4 gv[WJ], zv[WK];
+#pragma unroll
+        for (int i = 0; i < WJ; ++i) gv[i] = *reinterpret_cast<const float4*>(g_base + (size_t)i * j_step * RS + r);
+#pragma unroll
+        for (int i = 0; i < WK; ++i) zv[i] = *reinterpret_cast<const float4*>(z_base + (size_t)i * k_step * RS + r);
+#pragma unroll
+        for (int i = 0; i < WJ; ++i)
+#pragma unroll
+            for (int j = 0; j < WK; ++j) {
+                acc[i][j][0] = fmaf(gv[i].x, zv[j].x, acc[i][j][0]);
+                acc[i][j][1] = fmaf(gv[i].y, zv[j].y, acc[i][j][1]);
+                acc[i][j][0] = fmaf(gv[i].z, zv[j].z, acc[i][j][0]);
+                acc[i][j][1] = fmaf(gv[i].w, zv[j].w, acc[i][j][1]);
+            }
+    }
+}
+template <typename PairT>
+__device__ __forceinline__ auto wgrad_sum(const PairT (&v)[1]) {
+    const auto t = unpack2(v[0]);
+    return t.x + t.y;
+}
+__device__ __forceinline__ float wgrad_sum(const float (&v)[2]) { return v[0] + v[1]; }
 
 // WIDE: some net has more than K2_OUT_GROUP outputs (a separate instance: the <= 4-output code stays as it is)
 template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
 __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
-    typedef typename Pair<R>::type pair;
     constexpr int C = 1 + N1 + N2 + N3;
+    // plain float accumulators in the adjoint and weight-gradient GEMMs, except in the third-order instances: with them
+    // ptxas spills 16 B more in their WIDE instance, so those keep the point pairs (as the double instances do)
+    constexpr bool SCALAR_ACC = sizeof(R) == 4 && N3 == 0;
     constexpr int NT_COMPUTE = NTC, NT_TOTAL = NTC + 32, N_CWARPS = NTC / 32;
     extern __shared__ __align__(128) unsigned char smem[];
     const PjSpec& sp = A.spec;
@@ -287,13 +318,14 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                 }
                 // (2a) a_bar_{h-1} = W_l^T z_bar_h
                 const bool valid = u0 < HK;
-                pair acc[Q][C][P / 2];
+                typedef AdjAcc<R, P, SCALAR_ACC> AA;
+                typename AA::elem acc[Q][C][AA::n];
 #pragma unroll
                 for (int q = 0; q < Q; ++q)
 #pragma unroll
                     for (int c = 0; c < C; ++c)
 #pragma unroll
-                        for (int hh = 0; hh < P / 2; ++hh) acc[q][c][hh] = pair{};
+                        for (int hh = 0; hh < AA::n; ++hh) acc[q][c][hh] = typename AA::elem{};
                 const int rpc = chunk_elems(sizeof(R)) / HK;
                 for (int r0 = 0; r0 < HJ; r0 += rpc) {
                     const R* chunk = cur.acquire();
@@ -347,11 +379,14 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                     R* gw = gpart + net.w_off[l];
                     for (int wt = warp; wt < n_kb * n_jb; wt += N_CWARPS) {
                         const int jb = (wt / n_kb) * 32, kb = (wt % n_kb) * 32;
-                        pair wacc[WJ][WK];
+                        typedef AdjAcc<R, 2, SCALAR_ACC> WA;   // one point pair per output: two floats or one pair
+                        typename WA::elem wacc[WJ][WK][WA::n];
 #pragma unroll
                         for (int i = 0; i < WJ; ++i)
 #pragma unroll
-                            for (int jj = 0; jj < WK; ++jj) wacc[i][jj] = pair{};
+                            for (int jj = 0; jj < WK; ++jj)
+#pragma unroll
+                                for (int hh = 0; hh < WA::n; ++hh) wacc[i][jj][hh] = typename WA::elem{};
                         wgrad_tile(wacc, G + (size_t)(jb + jl) * RS, 4, Zb + (size_t)(kb + kl) * RS, 8, RS, C * T);
                         // every output element is owned by one thread of this CTA, so the fire-and-forget reduction
                         // (RED.ADD, no return value to wait for) into the CTA's private partial is race-free and ordered
@@ -362,8 +397,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                             for (int jj = 0; jj < WK; ++jj) {
                                 const int k = kb + kl + 8 * jj;
                                 if (j < width_j && k < width_k) {
-                                    const auto v = unpack2(wacc[i][jj]);
-                                    atomicAdd(&gw[(size_t)j * width_k + k], v.x + v.y);
+                                    atomicAdd(&gw[(size_t)j * width_k + k], wgrad_sum(wacc[i][jj]));
                                 }
                             }
                         }
