@@ -45,6 +45,9 @@ extern "C" {
 #define PJ_MAX_WIDTH 128  /* hidden width */
 #define PJ_ACT_TANH 0
 #define PJ_ACT_SIN 1
+#define PJ_ACT_SIGMOID 2  /* torch.nn.Sigmoid; this and the two below run on the FFMA kernels only           */
+#define PJ_ACT_SILU 3     /* torch.nn.SiLU, z sigmoid(z)                                                     */
+#define PJ_ACT_ELU 4      /* torch.nn.ELU with alpha = 1                                                     */
 
 /* One FCNN (reference networks.py:6-70): Linear, actv, ..., Linear. */
 typedef struct PjNet {
@@ -52,7 +55,7 @@ typedef struct PjNet {
     int32_t in_coord[PJ_MAX_COORDS];    /* input i is coordinate in_coord[i]  (conditions.py:52 torch.cat)    */
     int32_t n_linear;                   /* number of nn.Linear layers (>= 2)                                  */
     int32_t width[PJ_MAX_LINEAR + 1];   /* width[0]=n_in, width[l]=out_features of Linear l-1                 */
-    int32_t act;                        /* PJ_ACT_*                                                           */
+    int32_t act;                        /* PJ_ACT_*; the nets of one spec may mix them                        */
     int32_t yrow0;                      /* first row of this net in the jet table: row = yrow0 + o*C + c,     */
                                         /* C = 1 + n1 + n2 + n3                                               */
     int64_t w_off[PJ_MAX_LINEAR];       /* float offset of W_l (torch layout [out][in]) in theta / grad_theta */

@@ -50,16 +50,22 @@ def build(force=False, verbose=False, extra_flags=(), lib=None, objdir_name="bui
             (os.path.join(objdir, "optim.o"), os.path.join(HERE, "pinnjet_optim.cu"), list(extra_flags)),
             (os.path.join(objdir, "inst_common.o"), os.path.join(HERE, "pinnjet_inst.cu"),
              ["-DPJ_N1=-1", "-DPJ_N2=-1"] + list(extra_flags))]
-    for n1, n2, wl in SCHEMES:   # float kernels, then the double FFMA kernels of the same scheme (same source, PJ_F64=1)
-        for f64 in (0, 1):
-            jobs.append((os.path.join(objdir, f"inst_{n1}_{n2}_{wl}" + ("_f64" if f64 else "") + ".o"),
-                         os.path.join(HERE, "pinnjet_inst.cu"),
-                         [f"-DPJ_N1={n1}", f"-DPJ_N2={n2}", f"-DPJ_WL={wl}", f"-DPJ_F64={f64}"] + list(extra_flags)))
-    for n1, n2, wl, n3 in THIRD_ORDER_SCHEMES:
-        for f64 in (0, 1):
-            jobs.append((os.path.join(objdir, f"inst_{n1}_{n2}_{wl}_{n3}" + ("_f64" if f64 else "") + ".o"),
-                         os.path.join(HERE, "pinnjet_inst.cu"),
-                         [f"-DPJ_N1={n1}", f"-DPJ_N2={n2}", f"-DPJ_WL={wl}", f"-DPJ_N3={n3}", f"-DPJ_F64={f64}"] + list(extra_flags)))
+    # float kernels, then the double FFMA kernels of the same scheme (same source, PJ_F64=1); each once more with the
+    # extended activation rule (PJ_XACT=1: sigmoid, SiLU, ELU)
+    for xact in (0, 1):
+        tag = "_xact" if xact else ""
+        for n1, n2, wl in SCHEMES:
+            for f64 in (0, 1):
+                jobs.append((os.path.join(objdir, f"inst_{n1}_{n2}_{wl}" + ("_f64" if f64 else "") + tag + ".o"),
+                             os.path.join(HERE, "pinnjet_inst.cu"),
+                             [f"-DPJ_N1={n1}", f"-DPJ_N2={n2}", f"-DPJ_WL={wl}", f"-DPJ_F64={f64}"] +
+                             (["-DPJ_XACT=1"] if xact else []) + list(extra_flags)))
+        for n1, n2, wl, n3 in THIRD_ORDER_SCHEMES:
+            for f64 in (0, 1):
+                jobs.append((os.path.join(objdir, f"inst_{n1}_{n2}_{wl}_{n3}" + ("_f64" if f64 else "") + tag + ".o"),
+                             os.path.join(HERE, "pinnjet_inst.cu"),
+                             [f"-DPJ_N1={n1}", f"-DPJ_N2={n2}", f"-DPJ_WL={wl}", f"-DPJ_N3={n3}", f"-DPJ_F64={f64}"] +
+                             (["-DPJ_XACT=1"] if xact else []) + list(extra_flags)))
     logs = []
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         for out, rc, log in ex.map(_compile, jobs):

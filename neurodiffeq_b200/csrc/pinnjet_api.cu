@@ -21,7 +21,13 @@ namespace pj {
     int occupancy_##N1##_##N2##_##WL(const Plan& pl, int k, int smem);                                    \
     cudaError_t launch_k1_f64_##N1##_##N2##_##WL(const K1ArgsF64& a, int grid, int smem, cudaStream_t s); \
     cudaError_t launch_k2_f64_##N1##_##N2##_##WL(const K2ArgsF64& a, int grid, int smem, cudaStream_t s); \
-    int occupancy_f64_##N1##_##N2##_##WL(const Plan& pl, int k, int smem);
+    int occupancy_f64_##N1##_##N2##_##WL(const Plan& pl, int k, int smem);                                 \
+    cudaError_t launch_k1_xact_##N1##_##N2##_##WL(const K1Args& a, int grid, int smem, cudaStream_t s);   \
+    cudaError_t launch_k2_xact_##N1##_##N2##_##WL(const K2Args& a, int grid, int smem, cudaStream_t s);   \
+    int occupancy_xact_##N1##_##N2##_##WL(const Plan& pl, int k, int smem);                               \
+    cudaError_t launch_k1_f64_xact_##N1##_##N2##_##WL(const K1ArgsF64& a, int grid, int smem, cudaStream_t s); \
+    cudaError_t launch_k2_f64_xact_##N1##_##N2##_##WL(const K2ArgsF64& a, int grid, int smem, cudaStream_t s); \
+    int occupancy_f64_xact_##N1##_##N2##_##WL(const Plan& pl, int k, int smem);
 PJ_DECL(1, 0, 0)
 PJ_DECL(1, 1, 0)
 PJ_DECL(2, 0, 0)
@@ -51,17 +57,21 @@ template <> struct Kernels<double> {
     cudaError_t (*k2)(const K2ArgsF64&, int, int, cudaStream_t);
     int (*occ)(const Plan&, int, int);
 };
+// The kernels of one scheme: tanh / sine instances, and the instances with the extended activation rule (xact: sigmoid,
+// SiLU, ELU), which a spec selects when one of its nets has such an activation (uses_extended_activation).
 struct SchemeEntry {
     int n1, n2, wl, n3;
-    Kernels<float> f32;
-    Kernels<double> f64;
-    template <typename R> const Kernels<R>& of() const;
+    Kernels<float> f32, f32_xact;
+    Kernels<double> f64, f64_xact;
+    template <typename R> const Kernels<R>& of(bool xact) const;
 };
-template <> const Kernels<float>& SchemeEntry::of<float>() const { return f32; }
-template <> const Kernels<double>& SchemeEntry::of<double>() const { return f64; }
+template <> const Kernels<float>& SchemeEntry::of<float>(bool xact) const { return xact ? f32_xact : f32; }
+template <> const Kernels<double>& SchemeEntry::of<double>(bool xact) const { return xact ? f64_xact : f64; }
 #define PJ_ENTRY(N1, N2, WL, N3, NAME)                                                                                        \
     {N1, N2, WL, N3, {launch_k1_##NAME, launch_k2_##NAME, occupancy_##NAME},                                                  \
-     {launch_k1_f64_##NAME, launch_k2_f64_##NAME, occupancy_f64_##NAME}}
+     {launch_k1_xact_##NAME, launch_k2_xact_##NAME, occupancy_xact_##NAME},                                                   \
+     {launch_k1_f64_##NAME, launch_k2_f64_##NAME, occupancy_f64_##NAME},                                                      \
+     {launch_k1_f64_xact_##NAME, launch_k2_f64_xact_##NAME, occupancy_f64_xact_##NAME}}
 static const SchemeEntry kSchemes[] = {
     PJ_ENTRY(1, 0, 0, 0, 1_0_0), PJ_ENTRY(1, 1, 0, 0, 1_1_0), PJ_ENTRY(2, 0, 0, 0, 2_0_0), PJ_ENTRY(2, 1, 0, 0, 2_1_0),
     PJ_ENTRY(2, 2, 0, 0, 2_2_0), PJ_ENTRY(3, 0, 0, 0, 3_0_0), PJ_ENTRY(3, 3, 0, 0, 3_3_0), PJ_ENTRY(2, 1, 2, 0, 2_1_2),
@@ -102,7 +112,7 @@ static const SchemeEntry* find_scheme(const PjSpec& sp) {
 
 template <typename R>
 static int occupancy(const PjSpec& sp, const Plan& pl, int k, int smem) {
-    return find_scheme(sp)->of<R>().occ(pl, k, smem);
+    return find_scheme(sp)->of<R>(uses_extended_activation(sp)).occ(pl, k, smem);
 }
 
 // make_plan (pinnjet_plan.cpp) for the current device, the current value of PINNJET_TC and the kernels of element type R
@@ -399,7 +409,8 @@ static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, con
         if (rc != 0) return fail(-5, "cuLaunchKernelEx of the specialised forward kernel failed (%d)", rc);
         return 0;
     }
-    return check_cuda(e->of<R>().k1(a, a.plan.grid, a.plan.k1_bytes, (cudaStream_t)stream), "forward launch");
+    return check_cuda(e->of<R>(uses_extended_activation(*spec)).k1(a, a.plan.grid, a.plan.k1_bytes, (cudaStream_t)stream),
+                      "forward launch");
 }
 
 extern "C" {
@@ -474,7 +485,9 @@ static int run_k2(const PjSpec* spec, const R* const* coords, int64_t n_points, 
     a.wts = reinterpret_cast<const R*>(w + a.plan.ws_wts);
     a.dbg = reinterpret_cast<float*>(w + a.plan.ws_loss) + LOSS_DBG_WORD;
     const SchemeEntry* e = find_scheme(*spec);
-    if (int rc = check_cuda(e->of<R>().k2(a, a.plan.grid_bwd, a.plan.k2_bytes, (cudaStream_t)stream), "backward launch")) return rc;
+    if (int rc = check_cuda(e->of<R>(uses_extended_activation(*spec)).k2(a, a.plan.grid_bwd, a.plan.k2_bytes, (cudaStream_t)stream),
+                            "backward launch"))
+        return rc;
     *gpart = a.gpart;
     *n_parts = a.plan.grid_bwd;
     return 0;

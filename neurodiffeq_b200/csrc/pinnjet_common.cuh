@@ -327,16 +327,98 @@ __device__ __forceinline__ void act_d2(int act, double z0, double& a0, double& s
 __device__ __forceinline__ void sincos_r(float x, float* s, float* c) { sincosf(x, s, c); }
 __device__ __forceinline__ void sincos_r(double x, double* s, double* c) { sincos(x, s, c); }
 
+// ---- the extended activation rule (PJ_XACT instances: sigmoid, SiLU and ELU besides tanh and sine) ----------------------
+// Branch-free logistic sigmoid 1 / (1 + 2^(-x log2 e)) with ex2.approx / rcp.approx: ~2 ulp for |x| < 8 (the rounding of
+// the scaled argument adds |x| 2^-24 relative beyond that), absolute error below 2^-23 everywhere; saturates to exactly 0
+// and 1.  Straight-line code for the same reason as tanh_fast.
+__device__ __forceinline__ float sigmoid_fast(float x) {
+    float e;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * -1.4426950408889634f));
+    float r;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(e + 1.0f));
+    return r;
+}
+// double: libdevice exp (the quotient adds one rounding)
+__device__ __forceinline__ double sigmoid_r(double x) { return 1.0 / (1.0 + exp(-x)); }
+__device__ __forceinline__ float sigmoid_r(float x) { return sigmoid_fast(x); }
+__device__ __forceinline__ float tanh_r(float x) { return tanh_fast(x); }
+__device__ __forceinline__ double tanh_r(double x) { return tanh(x); }
+__device__ __forceinline__ float expm1_r(float x) { return expm1f(x); }
+__device__ __forceinline__ double expm1_r(double x) { return expm1(x); }
+
+// Does the record's channel 0 hold the activation's value (tanh, sigmoid, ELU) rather than z0 (sine, SiLU)?  The reverse
+// pass derives every derivative it needs from that one number.
+template <bool XA>
+__device__ __forceinline__ bool record_holds_value(int act) {
+    if constexpr (XA) return act == PJ_ACT_TANH || act == PJ_ACT_SIGMOID || act == PJ_ACT_ELU;
+    return act == PJ_ACT_TANH;
+}
+
+// Value a0 and derivatives s[1..K] (K = 2..4) of activation `act`, from z0 (REC = false: the forward kernel) or from the
+// record's channel 0 (REC = true: the reverse kernel; see record_holds_value).  With sg = sigmoid(z0) and sg_k its
+// derivatives: sigmoid s_k = sg_k, polynomials in sg; SiLU z0 sg(z0): s_k = k sg_(k-1) + z0 sg_k; ELU (alpha = 1): s_1 = 1,
+// s_k>1 = 0 for a0 >= 0, else every s_k = a0 + 1.  At z0 = 0 both branches give s_1 = 1; the higher derivatives are 0 there,
+// as torch's double backward of elu gives them.
+template <bool REC, int K, typename R>
+__device__ __forceinline__ void act_x(int act, R x, R& a0, R (&s)[K + 1]) {
+    static_assert(K >= 2 && K <= 4, "derivatives 1..2, 3 or 4");
+    if (act == PJ_ACT_TANH) {
+        a0 = REC ? x : tanh_r(x);
+        s[1] = fma(-a0, a0, R(1));
+        s[2] = R(-2) * a0 * s[1];
+        if constexpr (K >= 3) s[3] = R(-2) * s[1] * s[1] - R(2) * a0 * s[2];
+        if constexpr (K >= 4) s[4] = R(-6) * s[1] * s[2] - R(2) * a0 * s[3];
+    } else if (act == PJ_ACT_SIN) {
+        sincos_r(x, &a0, &s[1]);
+        s[2] = -a0;
+        if constexpr (K >= 3) s[3] = -s[1];
+        if constexpr (K >= 4) s[4] = a0;
+    } else if (act == PJ_ACT_ELU) {
+        a0 = REC ? x : (x > R(0) ? x : expm1_r(fmin(x, R(0))));
+        const bool pos = a0 >= R(0);
+        const R e = a0 + R(1);
+        s[1] = pos ? R(1) : e;
+#pragma unroll
+        for (int k = 2; k <= K; ++k) s[k] = pos ? R(0) : e;
+    } else {   // sigmoid, SiLU
+        const R sg = (REC && act == PJ_ACT_SIGMOID) ? x : sigmoid_r(x);
+        R d[K + 1];
+        d[1] = sg * (R(1) - sg);
+        const R h = fma(R(-2), sg, R(1));   // 1 - 2 sg
+        d[2] = d[1] * h;
+        if constexpr (K >= 3) d[3] = d[1] * fma(R(6) * sg, sg - R(1), R(1));    // 1 - 6 sg + 6 sg^2
+        if constexpr (K >= 4) d[4] = d[2] * fma(R(12) * sg, sg - R(1), R(1));   // (1 - 2 sg)(1 - 12 sg + 12 sg^2)
+        if (act == PJ_ACT_SIGMOID) {
+            a0 = sg;
+#pragma unroll
+            for (int k = 1; k <= K; ++k) s[k] = d[k];
+        } else {
+            a0 = x * sg;
+            s[1] = fma(x, d[1], sg);
+#pragma unroll
+            for (int k = 2; k <= K; ++k) s[k] = fma(x, d[k], R(k) * d[k - 1]);
+        }
+    }
+}
+
 // z-jet -> a-jet, in place.  WL > 0: the single second-order channel is the weighted combination L = sum_d w[d] D_d^2.
 // N3 > 0: channels 1+N1+N2+t (t < N3) are the pure thirds of direction t, a3 = s3 z1^3 + 3 s2 z1 z2 + s1 z3 (N3 <= N2:
-// direction t has its first and second channel).
-template <int N1, int N2, int WL, int N3, typename R>
+// direction t has its first and second channel).  XA: the extended rule (act_x); otherwise tanh and sine only.
+template <int N1, int N2, int WL, int N3, bool XA = false, typename R>
 __device__ __forceinline__ void act_forward(int act, R (&z)[1 + N1 + N2 + N3], const R* w) {
-    R a0, s1, s2;
-    act_d2(act, z[0], a0, s1, s2);
+    R a0, s1, s2, s3;
+    if constexpr (XA) {
+        R s[N3 > 0 ? 4 : 3];
+        act_x<false, (N3 > 0 ? 3 : 2)>(act, z[0], a0, s);
+        s1 = s[1];
+        s2 = s[2];
+        if constexpr (N3 > 0) s3 = s[3];
+    } else {
+        act_d2(act, z[0], a0, s1, s2);
+    }
     if constexpr (N3 > 0) {   // before the first- and second-order channels are overwritten
         static_assert(WL == 0 && N3 <= N2, "third-order channels need the pure second of their direction");
-        const R s3 = act == PJ_ACT_TANH ? R(-2) * s1 * s1 - R(2) * a0 * s2 : -s1;
+        if constexpr (!XA) s3 = act == PJ_ACT_TANH ? R(-2) * s1 * s1 - R(2) * a0 * s2 : -s1;
 #pragma unroll
         for (int t = 0; t < N3; ++t) {
             const R z1 = z[1 + t], z2 = z[1 + N1 + t];
@@ -360,12 +442,19 @@ __device__ __forceinline__ void act_forward(int act, R (&z)[1 + N1 + N2 + N3], c
 
 // reverse of the activation jet: given the stored record (channel 0 = tanh(z0) for tanh nets, z0 for sin nets; other
 // channels z-jets) and the adjoint of the a-jet, produce the a-jet (for the weight-gradient GEMM) and the adjoint of the
-// z-jet.
-template <int N1, int N2, int WL, int N3, typename R>
+// z-jet.  XA: the extended rule (act_x from the record: sigmoid(z0), z0 for SiLU, ELU(z0)).
+template <int N1, int N2, int WL, int N3, bool XA = false, typename R>
 __device__ __forceinline__ void act_backward(int act, const R (&z)[1 + N1 + N2 + N3], const R (&ab)[1 + N1 + N2 + N3],
                                              R (&a)[1 + N1 + N2 + N3], R (&zb)[1 + N1 + N2 + N3], const R* w) {
-    R a0, s1, s2, s3;
-    if (act == PJ_ACT_TANH) {   // record channel 0 = tanh(z0), stored by K1: no transcendental in the reverse pass
+    R a0, s1, s2, s3, s4;
+    if constexpr (XA) {
+        R s[N3 > 0 ? 5 : 4];
+        act_x<true, (N3 > 0 ? 4 : 3)>(act, z[0], a0, s);
+        s1 = s[1];
+        s2 = s[2];
+        s3 = s[3];
+        if constexpr (N3 > 0) s4 = s[4];
+    } else if (act == PJ_ACT_TANH) {   // record channel 0 = tanh(z0), stored by K1: no transcendental in the reverse pass
         a0 = z[0];
         s1 = fma(-a0, a0, R(1));
         s2 = R(-2) * a0 * s1;
@@ -405,7 +494,7 @@ __device__ __forceinline__ void act_backward(int act, const R (&z)[1 + N1 + N2 +
         }
     }
     if constexpr (N3 > 0) {   // reverse of a3 = s3 z1^3 + 3 s2 z1 z2 + s1 z3; s4 from the stored tanh(z0) or sin(z0)
-        const R s4 = act == PJ_ACT_TANH ? R(-6) * s1 * s2 - R(2) * a0 * s3 : a0;
+        if constexpr (!XA) s4 = act == PJ_ACT_TANH ? R(-6) * s1 * s2 - R(2) * a0 * s3 : a0;
 #pragma unroll
         for (int t = 0; t < N3; ++t) {
             const R z1 = z[1 + t], z2 = z[1 + N1 + t], z3 = z[1 + N1 + N2 + t], ab3 = ab[1 + N1 + N2 + t];

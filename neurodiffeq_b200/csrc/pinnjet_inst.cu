@@ -2,13 +2,19 @@
 // PJ_N1 = PJ_N2 = -1 builds the scheme-independent K2b reduce.  PJ_F64=1 builds the double FFMA kernels of the scheme
 // (launch_k1_f64_*, launch_k2_f64_*, occupancy_f64_*) from the same source; the tensor-core kernels are float only.
 // PJ_N3 > 0 (pure third-order channels) builds FFMA kernels only: the tensor-core kernels carry jets up to order 2.
+// PJ_XACT=1 builds the FFMA kernels of the scheme with the extended activation rule (sigmoid, SiLU and ELU besides tanh
+// and sine; launch_k1_xact_*, launch_k1_f64_xact_*, ...): the PJ_XACT=0 units, which every tanh / sine problem runs, keep
+// their code.
 #ifndef PJ_WL
 #define PJ_WL 0
 #endif
 #ifndef PJ_N3
 #define PJ_N3 0
 #endif
-#define PJ_TC_UNIT (!PJ_F64 && PJ_N3 == 0)
+#ifndef PJ_XACT
+#define PJ_XACT 0
+#endif
+#define PJ_TC_UNIT (!PJ_F64 && PJ_N3 == 0 && !PJ_XACT)
 
 #include "pinnjet_k1.cuh"
 #include "pinnjet_k2.cuh"
@@ -26,12 +32,24 @@
 #else
 #define PJ_NAME(prefix, n1, n2) PJ_NAME4(prefix, n1, n2, PJ_WL)
 #endif
-#if PJ_F64
+#if PJ_F64 && PJ_XACT
+#define PJ_PREFIX_K1 launch_k1_f64_xact_
+#define PJ_PREFIX_K2 launch_k2_f64_xact_
+#define PJ_PREFIX_OCC occupancy_f64_xact_
+#define PJ_K1_KERNEL k1_forward_kernel_f64_xact
+#define PJ_K2_KERNEL k2_backward_kernel_f64_xact
+#elif PJ_F64
 #define PJ_PREFIX_K1 launch_k1_f64_
 #define PJ_PREFIX_K2 launch_k2_f64_
 #define PJ_PREFIX_OCC occupancy_f64_
 #define PJ_K1_KERNEL k1_forward_kernel_f64
 #define PJ_K2_KERNEL k2_backward_kernel_f64
+#elif PJ_XACT
+#define PJ_PREFIX_K1 launch_k1_xact_
+#define PJ_PREFIX_K2 launch_k2_xact_
+#define PJ_PREFIX_OCC occupancy_xact_
+#define PJ_K1_KERNEL k1_forward_kernel_xact
+#define PJ_K2_KERNEL k2_backward_kernel_xact
 #else
 #define PJ_PREFIX_K1 launch_k1_
 #define PJ_PREFIX_K2 launch_k2_

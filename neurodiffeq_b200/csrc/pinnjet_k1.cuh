@@ -70,8 +70,9 @@ struct RingCursor {
 };
 
 // z-jets of P points of one unit (registers) -> workspace record (train), activation-jet rule, a-jets -> shared memory.
-// Record channel 0 holds tanh(z0) for tanh nets (the reverse pass then needs no transcendental) and z0 for sin nets.
-template <int P, int N1, int N2, int WL, int N3, typename R>
+// Record channel 0 holds tanh(z0) for tanh nets (the reverse pass then needs no transcendental) and z0 for sin nets;
+// XA instances: see record_holds_value.
+template <int P, int N1, int N2, int WL, int N3, bool XA, typename R>
 __device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2 + N3], int act_kind, R* __restrict__ act_row, int T,
                                             R* __restrict__ rec_row, int T2, const R (&wq)[P][WL > 0 ? WL : 1]) {
     constexpr int C = 1 + N1 + N2 + N3;
@@ -89,9 +90,9 @@ __device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2 + N3], int ac
         for (int c = 1; c < C; ++c) store(rec_row + c * T2, zq, c);
     }
 #pragma unroll
-    for (int p = 0; p < P; ++p) act_forward<N1, N2, WL, N3>(act_kind, zq[p], wq[p]);
+    for (int p = 0; p < P; ++p) act_forward<N1, N2, WL, N3, XA>(act_kind, zq[p], wq[p]);
     if (rec_row) {
-        if (act_kind == PJ_ACT_TANH) {
+        if (record_holds_value<XA>(act_kind)) {
 #pragma unroll
             for (int p = 0; p < P; ++p) z0s[p] = zq[p][0];
         }
@@ -104,7 +105,7 @@ __device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2 + N3], int ac
     for (int c = 0; c < C; ++c) store(act_row + c * T, zq, c);
 }
 
-template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3>
+template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3, bool XA>
 __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
     typedef typename Pair<R>::type pair;
     constexpr int C = 1 + N1 + N2 + N3;
@@ -284,7 +285,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
 #pragma unroll
                             for (int s2 = 0; s2 < N2 + N3; ++s2) zq[p][1 + N1 + s2] = 0.0f;   // second and third orders: 0
                         }
-                        finish_unit<P, N1, N2, WL, N3>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
+                        finish_unit<P, N1, N2, WL, N3, XA>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
                     }
                 }
             }
@@ -323,7 +324,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
                         for (int c = 0; c < C; ++c)
 #pragma unroll
                             for (int p = 0; p < P; ++p) zq[p][c] = pick<P>(acc[q][c], p) + (c == 0 ? bias : 0.0f);
-                        finish_unit<P, N1, N2, WL, N3>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
+                        finish_unit<P, N1, N2, WL, N3, XA>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
                     }
                 }
                 bar_compute<NTC>();
@@ -365,14 +366,24 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
     PJ_T_FLUSH(0)
 }
 
-// The float and double kernels: one body (element type R); the float instance keeps its name and argument type.
+// The float and double kernels: one body (element type R); the float instance keeps its name and argument type.  The
+// _xact kernels carry the extended activation rule (sigmoid, SiLU, ELU): instances of their own, so that the tanh / sine
+// kernels keep their code.
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3>
 __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel(const __grid_constant__ K1Args A) {
-    k1_forward_body<float, NTC, P, Q, N1, N2, WL, N3>(A);
+    k1_forward_body<float, NTC, P, Q, N1, N2, WL, N3, false>(A);
 }
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3>
 __global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel_f64(const __grid_constant__ K1ArgsF64 A) {
-    k1_forward_body<double, NTC, P, Q, N1, N2, WL, N3>(A);
+    k1_forward_body<double, NTC, P, Q, N1, N2, WL, N3, false>(A);
+}
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3>
+__global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel_xact(const __grid_constant__ K1Args A) {
+    k1_forward_body<float, NTC, P, Q, N1, N2, WL, N3, true>(A);
+}
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3>
+__global__ void __launch_bounds__(ffma_k1_threads(NTC), MINB) k1_forward_kernel_f64_xact(const __grid_constant__ K1ArgsF64 A) {
+    k1_forward_body<double, NTC, P, Q, N1, N2, WL, N3, true>(A);
 }
 
 }  // namespace pj

@@ -69,8 +69,9 @@ __device__ __forceinline__ auto wgrad_sum(const PairT (&v)[1]) {
 }
 __device__ __forceinline__ float wgrad_sum(const float (&v)[2]) { return v[0] + v[1]; }
 
-// WIDE: some net has more than K2_OUT_GROUP outputs (a separate instance: the <= 4-output code stays as it is)
-template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
+// WIDE: some net has more than K2_OUT_GROUP outputs (a separate instance: the <= 4-output code stays as it is).  XA: the
+// extended activation rule (act_x).
+template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE, bool XA>
 __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     constexpr int C = 1 + N1 + N2 + N3;
     // plain float accumulators in the adjoint and weight-gradient GEMMs, except in the third-order instances: with them
@@ -193,7 +194,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
 #pragma unroll
                                     for (int c = 0; c < C; ++c) ab[c] = fma(w, ybar[(o * C + c) * T + pt], ab[c]);
                                 }
-                            act_backward<N1, N2, WL, N3>(act_kind, z, ab, a, zb, wq[p]);
+                            act_backward<N1, N2, WL, N3, XA>(act_kind, z, ab, a, zb, wq[p]);
 #pragma unroll
                             for (int o = 0; o < K2_OUT_GROUP; ++o)
                                 if (o < n_out) {
@@ -247,7 +248,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
 #pragma unroll
                                 for (int c = 0; c < C; ++c) ab[c] = fma(w, ybar[(o * C + c) * T + pt], ab[c]);
                             }
-                            act_backward<N1, N2, WL, N3>(act_kind, z, ab, a, zb, wq[p]);
+                            act_backward<N1, N2, WL, N3, XA>(act_kind, z, ab, a, zb, wq[p]);
                             gb += zb[0];
 #pragma unroll
                             for (int c = 0; c < C; ++c) {
@@ -352,7 +353,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                                 z[c] = Zb[u * RS + c * T + p0 + p];
                                 ab[c] = pick<P>(acc[q][c], p);
                             }
-                            act_backward<N1, N2, WL, N3>(act_kind, z, ab, av[p], zv[p], wq[p]);
+                            act_backward<N1, N2, WL, N3, XA>(act_kind, z, ab, av[p], zv[p], wq[p]);
                             gb += zv[p][0];
                         }
 #pragma unroll
@@ -489,14 +490,23 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     }
 }
 
-// The float and double kernels: one body (element type R); the float instance keeps its name and argument type.
+// The float and double kernels: one body (element type R); the float instance keeps its name and argument type.  The
+// _xact kernels carry the extended activation rule (as in pinnjet_k1.cuh).
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
 __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
-    k2_backward_body<float, NTC, P, Q, N1, N2, WL, N3, WIDE>(A);
+    k2_backward_body<float, NTC, P, Q, N1, N2, WL, N3, WIDE, false>(A);
 }
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
 __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel_f64(const __grid_constant__ K2ArgsF64 A) {
-    k2_backward_body<double, NTC, P, Q, N1, N2, WL, N3, WIDE>(A);
+    k2_backward_body<double, NTC, P, Q, N1, N2, WL, N3, WIDE, false>(A);
+}
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
+__global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel_xact(const __grid_constant__ K2Args A) {
+    k2_backward_body<float, NTC, P, Q, N1, N2, WL, N3, WIDE, true>(A);
+}
+template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
+__global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel_f64_xact(const __grid_constant__ K2ArgsF64 A) {
+    k2_backward_body<double, NTC, P, Q, N1, N2, WL, N3, WIDE, true>(A);
 }
 
 }  // namespace pj

@@ -22,6 +22,12 @@ static int max_outputs(const PjSpec& sp) {   // widest output Linear of all nets
     return m;
 }
 
+bool uses_extended_activation(const PjSpec& sp) {
+    for (int i = 0; i < sp.n_nets && i < PJ_MAX_NETS_ALL; ++i)
+        if (net_of(sp, i).act != PJ_ACT_TANH && net_of(sp, i).act != PJ_ACT_SIN) return true;
+    return false;
+}
+
 static int hidden_linears(const PjSpec& sp) {   // hidden->hidden Linears of all nets
     int n = 0;
     for (int i = 0; i < sp.n_nets; ++i) n += net_of(sp, i).n_linear - 2;
@@ -167,7 +173,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
         if (net.n_in < 1 || net.n_in > PJ_MAX_COORDS || net.width[0] != net.n_in) return fail(-1, "net %d: bad n_in", n);
         const int n_out = net.width[net.n_linear];
         if (n_out < 1 || n_out > PJ_MAX_OUT) return fail(-2, "net %d: %d output units (max %d)", n, n_out, PJ_MAX_OUT);
-        if (net.act != PJ_ACT_TANH && net.act != PJ_ACT_SIN) return fail(-2, "net %d: unknown activation", n);
+        if (net.act < PJ_ACT_TANH || net.act > PJ_ACT_ELU) return fail(-2, "net %d: unknown activation", n);
         if (net.yrow0 != yrows) return fail(-1, "net %d: yrow0 must be %d", n, yrows);
         yrows += n_out * C;
         pl.hp[n][0] = net.n_in;
@@ -246,10 +252,11 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     // ---- kernel selection ----
     // Tensor-core kernels (pinnjet_tc.cuh): every hidden layer exactly 64 wide (after padding), at most 8 jet channels, at
     // most 4 outputs per net (one 16-byte row of the output Linear), no third-order channels, at most PJ_MAX_NETS network
-    // instances (their register arrays are sized by it), the weight images of both kernels resident in shared memory.  The
-    // decision may not depend on the program length (only pj_forward* know it): the programs get a fixed reserve.
+    // instances (their register arrays are sized by it), tanh and sine only, the weight images of both kernels resident in
+    // shared memory.  The decision may not depend on the program length (only pj_forward* know it): the programs get a
+    // fixed reserve.
     bool tc = esz == 4 && dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4 && sp.n3 == 0 &&
-              sp.n_nets <= PJ_MAX_NETS;
+              sp.n_nets <= PJ_MAX_NETS && !uses_extended_activation(sp);
     for (int n = 0; tc && n < sp.n_nets; ++n)
         for (int h = 1; h < net_of(sp, n).n_linear; ++h) tc = tc && pl.hp[n][h] == TC_H;
     if (tc) {   // both kernels tile like the forward kernel; seeds / weights / records are shared as is

@@ -140,6 +140,10 @@ struct PlanDevice {
     int (*occupancy)(const PjSpec& sp, const Plan& pl, int k, int smem);
 };
 
+// Does some net of the spec use an activation other than tanh and sine?  Such a spec runs the FFMA instances with the
+// extended activation rule (PJ_XACT), never the tensor-core kernels.
+bool uses_extended_activation(const PjSpec& sp);
+
 // 0 or a negative code with a message in err[0, err_len): -1 invalid spec / arguments, -2 the kernels cannot take the
 // problem, -3 internal inconsistency, -4 the device query failed.  prog_len / prog_w_len move only the K1 image.
 // esz = 8 plans the double kernels: always FFMA (whatever dev.tc_level says), every buffer of 8-byte elements, at most

@@ -3,7 +3,8 @@
 ``FCNN`` keeps the reference's module layout -- an ``nn.Sequential`` called ``NN`` of ``Linear, actv, ..., Linear`` with
 parameters at ``NN.{0,2,4,...}.{weight,bias}`` -- so state dicts, optimizers, checkpoints and ``deepcopy`` of user code
 keep working; the CUDA engine reads the weights of exactly this structure (any ``nn.Sequential`` alternating
-``nn.Linear`` with ``nn.Tanh`` / ``SinActv`` is accepted, see ``engine.describe_network``).
+``nn.Linear`` with ``nn.Tanh`` / ``SinActv`` / ``nn.Sigmoid`` / ``nn.SiLU`` / ``nn.ELU`` (alpha = 1) is accepted, see
+``tracing.NetDescription``).
 """
 from warnings import warn
 

@@ -15,7 +15,10 @@ import torch.nn as nn
 from . import symbolic as S
 from .networks import SinActv
 
-ACT_TANH, ACT_SIN = 0, 1
+ACT_TANH, ACT_SIN, ACT_SIGMOID, ACT_SILU, ACT_ELU = 0, 1, 2, 3, 4   # PJ_ACT_* of include/pinnjet.h
+# torch modules with a jet rule in the kernels, matched by exact type: a subclass may compute something else (the
+# product's own Swish(beta=1) equals SiLU but stays on the autograd path with its trainable-scalar variants)
+_TORCH_ACTS = {nn.Sigmoid: ACT_SIGMOID, nn.SiLU: ACT_SILU, nn.ELU: ACT_ELU}
 
 
 def check_jet_order(jet_order):
@@ -63,9 +66,13 @@ class NetDescription:
                 kinds.add(ACT_TANH)
             elif isinstance(a, SinActv) or type(a).__name__ == "SinActv":
                 kinds.add(ACT_SIN)
+            elif type(a) in _TORCH_ACTS:
+                if type(a) is nn.ELU and a.alpha != 1.0:
+                    raise NotImplementedError(f"nn.ELU(alpha={a.alpha}) has no jet rule in the fused kernels (alpha = 1 only)")
+                kinds.add(_TORCH_ACTS[type(a)])
             else:
                 raise NotImplementedError(f"activation {type(a).__name__} has no jet rule in the fused kernels "
-                                          f"(implemented: nn.Tanh, SinActv)")
+                                          f"(implemented: nn.Tanh, SinActv, nn.Sigmoid, nn.SiLU, nn.ELU with alpha=1)")
         if len(kinds) != 1:
             raise NotImplementedError("all hidden activations of one network must be the same")
         self.act = kinds.pop()

@@ -153,9 +153,10 @@ def _c5(nd):
 # Extension workloads (SURVEY.md §8f.2): conditions with Neumann data, which evaluate the network AT a boundary abscissa
 # (reference conditions.py:585-596, 823-834).  Not BASELINE configs -- parity cases for the widened condition family.
 # ----------------------------------------------------------------------------------------------------------------------
-def _heat(nd, name, neumann_side):
+def _heat(nd, name, neumann_side, width=64, actv=None, act_name="tanh"):
     def make_nets():
-        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(64, 64))]
+        kw = {} if actv is None else {"actv": actv}
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(width, width), **kw)]
 
     def make_conditions():
         kw = dict(x_min=0.0, x_max=1.0, t_min=0.0, t_min_val=lambda x: torch.sin(0.5 * np.pi * x))
@@ -170,8 +171,9 @@ def _heat(nd, name, neumann_side):
     def diff_eqs(u, x, t):
         return [nd.diff(u, t) - 0.3 * nd.diff(u, x, order=2)]
 
-    return Workload(name, "Solver2D", ("x", "t"), ((0.0, 1.0), (0.0, 1.0)), [((2, 64, 64, 1), "tanh")], make_nets,
-                    make_conditions, diff_eqs, 1, 16384, 2 * _fcnn_flops((2, 64, 64, 1), 9), None)
+    shape = (2, width, width, 1)
+    return Workload(name, "Solver2D", ("x", "t"), ((0.0, 1.0), (0.0, 1.0)), [(shape, act_name)], make_nets,
+                    make_conditions, diff_eqs, 1, 16384, 2 * _fcnn_flops(shape, 9), None)
 
 
 def _bvp(nd, name, kw):
@@ -273,11 +275,12 @@ def _biharmonic(nd):
 # ----------------------------------------------------------------------------------------------------------------------
 # T1, T2  pure third derivatives of a network output: the fused kernels' third-order channels (jet_order=3)
 # ----------------------------------------------------------------------------------------------------------------------
-def _kdv(nd):
+def _kdv(nd, name="t1_kdv", actv=None, act_name="tanh"):
     """Korteweg-de Vries  u_t + 6 u u_x + u_xxx = 0  on [-1, 1] x [0, 1] (IBVP1D, Dirichlet ends): channels (x, t) firsts,
     x second and third; a 64-wide network, which the tensor-core kernels would otherwise take."""
     def make_nets():
-        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(64, 64))]
+        kw = {} if actv is None else {"actv": actv}
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(64, 64), **kw)]
 
     def make_conditions():
         return [nd.IBVP1D(x_min=-1, x_max=1, t_min=0, t_min_val=lambda x: -torch.sin(np.pi * x),
@@ -286,7 +289,7 @@ def _kdv(nd):
     def diff_eqs(u, x, t):
         return [nd.diff(u, t) + 6 * u * nd.diff(u, x) + nd.diff(u, x, order=3)]
 
-    return Workload("t1_kdv", "Solver2D", ("x", "t"), ((-1.0, 1.0), (0.0, 1.0)), [((2, 64, 64, 1), "tanh")], make_nets,
+    return Workload(name, "Solver2D", ("x", "t"), ((-1.0, 1.0), (0.0, 1.0)), [((2, 64, 64, 1), act_name)], make_nets,
                     make_conditions, diff_eqs, 1, 16384, _fcnn_flops((2, 64, 64, 1), 5), None)
 
 
@@ -451,6 +454,54 @@ def _m3(nd):
                     16384, sum(_fcnn_flops(w, 2) for w, _ in shapes), None)
 
 
+# ----------------------------------------------------------------------------------------------------------------------
+# A1..A4  torch activations with a jet rule of the extended kernel instances: nn.Sigmoid, nn.SiLU, nn.ELU (alpha = 1)
+# ----------------------------------------------------------------------------------------------------------------------
+def _a1(nd):
+    """The nonlinear Poisson problem of the reference's getting-started notebook (`de_star`) on an ELU network of width 40
+    (padded to 64 in the kernels): u_xx + u_yy + exp(u) - 1 - x^2 - y^2 - 4 / (1 + x^2 + y^2)^2 = 0, posed here on
+    [-1, 1]^2 (DirichletBVP2D) with the exact solution log(1 + x^2 + y^2) as boundary data."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(40, 40), actv=torch.nn.ELU)]
+
+    def make_conditions():
+        return [nd.DirichletBVP2D(
+            x_min=-1, x_min_val=lambda y: torch.log(2 + y ** 2),
+            x_max=1, x_max_val=lambda y: torch.log(2 + y ** 2),
+            y_min=-1, y_min_val=lambda x: torch.log(2 + x ** 2),
+            y_max=1, y_max_val=lambda x: torch.log(2 + x ** 2),
+        )]
+
+    def diff_eqs(u, x, y):
+        return [nd.diff(u, x, order=2) + nd.diff(u, y, order=2) + torch.exp(u) - 1.0 - x ** 2 - y ** 2
+                - 4.0 / (1.0 + x ** 2 + y ** 2) ** 2]
+
+    return Workload("a1_de_star_elu", "Solver2D", ("x", "y"), ((-1.0, 1.0), (-1.0, 1.0)), [((2, 40, 40, 1), "elu")],
+                    make_nets, make_conditions, diff_eqs, 1, 16384, _fcnn_flops((2, 40, 40, 1), 4), None)
+
+
+def _a4(nd):
+    """SIR epidemic model, one network per compartment with three activations (nn.Tanh, nn.Sigmoid, nn.ELU): one launch
+    mixes the tanh rule and the extended ones."""
+    beta, gamma = 1.5, 0.4
+    acts = (torch.nn.Tanh, torch.nn.Sigmoid, torch.nn.ELU)
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(32, 32), actv=a) for a in acts]
+
+    def make_conditions():
+        return [nd.IVP(t_0=0.0, u_0=v) for v in (0.99, 0.01, 0.0)]
+
+    def diff_eqs(s, i, r, t):
+        return [nd.diff(s, t) + beta * s * i,
+                nd.diff(i, t) - beta * s * i + gamma * i,
+                nd.diff(r, t) - gamma * i]
+
+    return Workload("a4_sir_mixed_activations", "Solver1D", ("t",), ((0.0, 10.0),),
+                    [((1, 32, 32, 1), a) for a in ("tanh", "sigmoid", "elu")], make_nets, make_conditions, diff_eqs, 3,
+                    32768, 3 * _fcnn_flops((1, 32, 32, 1), 2), None)
+
+
 _EXTRA = {
     "x1": lambda nd: _heat(nd, "x1_heat_dirichlet_neumann", "right"),
     "x2": lambda nd: _heat(nd, "x2_heat_neumann_dirichlet", "left"),
@@ -482,6 +533,15 @@ _BUILDERS.update(_THIRD_ORDER)
 _SYSTEM = {"m1": _m1, "m2": _m2, "m3": _m3}
 SYSTEM_NAMES = tuple(_SYSTEM)
 _BUILDERS.update(_SYSTEM)
+# nn.Sigmoid / nn.SiLU / nn.ELU networks (a3 with jet_order=3); kept out of the tuples above as well
+_ACTIVATION = {
+    "a1": _a1,
+    "a2": lambda nd: _heat(nd, "a2_heat_neumann_sigmoid", "right", width=32, actv=torch.nn.Sigmoid, act_name="sigmoid"),
+    "a3": lambda nd: _kdv(nd, "a3_kdv_silu", actv=torch.nn.SiLU, act_name="silu"),
+    "a4": _a4,
+}
+ACTIVATION_NAMES = tuple(_ACTIVATION)
+_BUILDERS.update(_ACTIVATION)
 # workloads whose conditions see only the first coordinate (a network of r alone, as SolverSpherical passes it)
 _RADIAL = ("s1", "s2")
 
