@@ -39,7 +39,8 @@ extern "C" {
 #define PJ_MAX_NETS 4      /* network instances in PjSpec.net (the tensor-core kernels take at most this many)  */
 #define PJ_MAX_NETS_ALL 16 /* network instances per problem: net[0..3], then net_more[0..11] (FFMA kernels)  */
 #define PJ_MAX_OUT 32     /* output units per network (the tensor-core kernels take at most 4) */
-#define PJ_MAX_LINEAR 8   /* nn.Linear layers per network (hidden layers + 1) */
+#define PJ_MAX_LINEAR 8   /* nn.Linear layers a PjNet describes by itself (hidden layers + 1) */
+#define PJ_MAX_LINEAR_ALL 16 /* nn.Linear layers per network: PjNet, then the network's PjNetDeep (FFMA kernels)  */
 #define PJ_MAX_COORDS 8
 #define PJ_MAX_DIRS 4     /* first-order jet directions */
 #define PJ_MAX_WIDTH 128  /* hidden width */
@@ -53,14 +54,22 @@ extern "C" {
 typedef struct PjNet {
     int32_t n_in;                       /* network inputs                                                    */
     int32_t in_coord[PJ_MAX_COORDS];    /* input i is coordinate in_coord[i]  (conditions.py:52 torch.cat)    */
-    int32_t n_linear;                   /* number of nn.Linear layers (>= 2)                                  */
-    int32_t width[PJ_MAX_LINEAR + 1];   /* width[0]=n_in, width[l]=out_features of Linear l-1                 */
+    int32_t n_linear;                   /* number of nn.Linear layers (2..PJ_MAX_LINEAR_ALL)                  */
+    int32_t width[PJ_MAX_LINEAR + 1];   /* width[0]=n_in, width[l]=out_features of Linear l-1 (l > 8: deep)   */
     int32_t act;                        /* PJ_ACT_*; the nets of one spec may mix them                        */
     int32_t yrow0;                      /* first row of this net in the jet table: row = yrow0 + o*C + c,     */
                                         /* C = 1 + n1 + n2 + n3                                               */
     int64_t w_off[PJ_MAX_LINEAR];       /* float offset of W_l (torch layout [out][in]) in theta / grad_theta */
     int64_t b_off[PJ_MAX_LINEAR];       /* float offset of b_l                                                */
 } PjNet;
+
+/* Layers 9..16 of a network with more than PJ_MAX_LINEAR Linear layers: width[i] is width[PJ_MAX_LINEAR + 1 + i] of the
+ * network, w_off[i] / b_off[i] are those of Linear PJ_MAX_LINEAR + i.  Read through the PJ_NET_* accessors below. */
+typedef struct PjNetDeep {
+    int32_t width[PJ_MAX_LINEAR_ALL - PJ_MAX_LINEAR];
+    int64_t w_off[PJ_MAX_LINEAR_ALL - PJ_MAX_LINEAR];
+    int64_t b_off[PJ_MAX_LINEAR_ALL - PJ_MAX_LINEAR];
+} PjNetDeep;
 
 /* Static problem description extracted once by the host (neurodiffeq_b200/tracing.py). */
 typedef struct PjSpec {
@@ -83,11 +92,24 @@ typedef struct PjSpec {
                                         /* zero-initialised spec of an older caller means what it meant       */
     PjNet net_more[PJ_MAX_NETS_ALL - PJ_MAX_NETS];   /* instances 4..n_nets-1.  Read only when n_nets > 4, so a  */
                                         /* caller whose struct ends at n3 keeps working with up to 4 nets     */
+    PjNetDeep deep[PJ_MAX_NETS_ALL];    /* layers 9..16 of instance n (n_linear > PJ_MAX_LINEAR).  Read only  */
+                                        /* when some instance has n_linear > PJ_MAX_LINEAR, so a caller whose */
+                                        /* struct ends at net_more keeps working with up to 8 Linear layers   */
 } PjSpec;
 
 /* Network instance n (0 <= n < n_nets) of a spec: net[n], then net_more[n - PJ_MAX_NETS].  A macro, so that host code, device
  * code and C callers share it (it evaluates n more than once). */
 #define PJ_SPEC_NET(spec, n) ((n) < PJ_MAX_NETS ? &(spec)->net[(n)] : &(spec)->net_more[(n) - PJ_MAX_NETS])
+
+/* Width of layer l (0 <= l <= n_linear: 0 the inputs, n_linear the outputs) and offsets of Linear l (0 <= l < n_linear) of a
+ * network given by its PjNet `net` and its PjNetDeep `deep` (pointers); the PJ_SPEC_* forms take instance n of a spec.
+ * Macros, for host code, device code and C callers alike (they evaluate their arguments more than once). */
+#define PJ_NET_WIDTH(net, deep, l) ((l) <= PJ_MAX_LINEAR ? (net)->width[(l)] : (deep)->width[(l) - PJ_MAX_LINEAR - 1])
+#define PJ_NET_W_OFF(net, deep, l) ((l) < PJ_MAX_LINEAR ? (net)->w_off[(l)] : (deep)->w_off[(l) - PJ_MAX_LINEAR])
+#define PJ_NET_B_OFF(net, deep, l) ((l) < PJ_MAX_LINEAR ? (net)->b_off[(l)] : (deep)->b_off[(l) - PJ_MAX_LINEAR])
+#define PJ_SPEC_WIDTH(spec, n, l) PJ_NET_WIDTH(PJ_SPEC_NET(spec, n), &(spec)->deep[(n)], l)
+#define PJ_SPEC_W_OFF(spec, n, l) PJ_NET_W_OFF(PJ_SPEC_NET(spec, n), &(spec)->deep[(n)], l)
+#define PJ_SPEC_B_OFF(spec, n, l) PJ_NET_B_OFF(PJ_SPEC_NET(spec, n), &(spec)->deep[(n)], l)
 
 /* Sizes the caller needs to allocate buffers (all bytes; workspace contents are opaque). */
 typedef struct PjSizes {

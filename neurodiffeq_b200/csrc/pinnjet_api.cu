@@ -88,13 +88,39 @@ static int fail(int code, const char* fmt, ...) {
     return code;
 }
 
-// The caller's spec as a kernel argument.  A caller built against a header whose PjSpec ends at n3 passes a shorter struct:
-// net_more is read only when the spec says it is there (n_nets > PJ_MAX_NETS), and is zero in the copy otherwise.
+// Some instance of the spec has more than PJ_MAX_LINEAR Linear layers: the spec has (and needs) its `deep` block.
+static bool has_deep_nets(const PjSpec& sp) {
+    for (int n = 0; n < sp.n_nets && n < PJ_MAX_NETS_ALL; ++n)
+        if (PJ_SPEC_NET(&sp, n)->n_linear > PJ_MAX_LINEAR) return true;
+    return false;
+}
+
+// The caller's spec as a kernel argument.  A caller built against an older header passes a shorter struct: net_more is
+// read only when the spec says it is there (n_nets > PJ_MAX_NETS), deep only when some instance is deeper than
+// PJ_MAX_LINEAR; what is not read is zero in the copy.
 static void copy_spec(PjSpec& dst, const PjSpec& src) {
-    const size_t head = offsetof(PjSpec, net_more);
-    const bool more = src.n_nets > PJ_MAX_NETS;
-    memcpy(&dst, &src, more ? sizeof(PjSpec) : head);
-    if (!more) memset(reinterpret_cast<char*>(&dst) + head, 0, sizeof(PjSpec) - head);
+    const size_t len = has_deep_nets(src) ? sizeof(PjSpec)
+                       : src.n_nets > PJ_MAX_NETS ? offsetof(PjSpec, deep) : offsetof(PjSpec, net_more);
+    memcpy(&dst, &src, len);
+    memset(reinterpret_cast<char*>(&dst) + len, 0, sizeof(PjSpec) - len);
+}
+
+// Instance n of a spec as the FFMA kernels index it
+static KNet kernel_net(const PjSpec& sp, int n) {
+    const PjNet& net = *PJ_SPEC_NET(&sp, n);
+    KNet k;
+    memset(&k, 0, sizeof(k));
+    k.n_in = net.n_in;
+    memcpy(k.in_coord, net.in_coord, sizeof(k.in_coord));
+    k.n_linear = net.n_linear;
+    k.act = net.act;
+    k.yrow0 = net.yrow0;
+    for (int l = 0; l <= net.n_linear && l <= PJ_MAX_LINEAR_ALL; ++l) k.width[l] = PJ_SPEC_WIDTH(&sp, n, l);
+    for (int l = 0; l < net.n_linear && l < PJ_MAX_LINEAR_ALL; ++l) {
+        k.w_off[l] = PJ_SPEC_W_OFF(&sp, n, l);
+        k.b_off[l] = PJ_SPEC_B_OFF(&sp, n, l);
+    }
+    return k;
 }
 
 static const SchemeEntry* find_scheme(const PjSpec& sp) {
@@ -151,10 +177,12 @@ __device__ void pack_bf16x3_image(unsigned char* img, const float* W, int rows, 
     }
 }
 
-// Grid (n_nets * PJ_MAX_LINEAR, PACK_PARTS): block (x, y) does every PACK_PARTS-th element of Linear x % PJ_MAX_LINEAR of net
-// x / PJ_MAX_LINEAR (4 CTAs per layer instead of 1: the kernel is latency bound).  All blocks together also clear
+// Grid (n_nets * S, PACK_PARTS), S = pack_stride(spec): block (x, y) does every PACK_PARTS-th element of Linear x % S of net
+// x / S (4 CTAs per layer instead of 1: the kernel is latency bound).  All blocks together also clear
 // zero_buf[0, n_zero) when given (pj_pack_zero: the optimizer.zero_grad() of the step rides along instead of a fill launch).
 constexpr int PACK_PARTS = 4;
+// blocks per net: PJ_MAX_LINEAR, or PJ_MAX_LINEAR_ALL when some net is deeper (shallow specs keep the smaller grid)
+static int pack_stride(const PjSpec& sp) { return has_deep_nets(sp) ? PJ_MAX_LINEAR_ALL : PJ_MAX_LINEAR; }
 
 template <typename R>
 __global__ void pack_kernel(const __grid_constant__ PackArgs A, const R* __restrict__ theta, R* __restrict__ pack,
@@ -168,14 +196,16 @@ __global__ void pack_kernel(const __grid_constant__ PackArgs A, const R* __restr
         for (long long i = ((long long)blockIdx.y * gridDim.x + blockIdx.x) * blockDim.x + threadIdx.x; i < n_zero; i += nthreads)
             zero_buf[i] = 0.0f;
     }
-    const int n = blockIdx.x / PJ_MAX_LINEAR, l = blockIdx.x % PJ_MAX_LINEAR;
+    const int stride = gridDim.x / sp.n_nets;   // pack_stride
+    const int n = blockIdx.x / stride, l = blockIdx.x % stride;
     if (n >= sp.n_nets) return;
     const PjNet& net = *PJ_SPEC_NET(&sp, n);
+    const PjNetDeep& deep = sp.deep[n];
     const int L = net.n_linear - 1;
     if (l > L) return;
-    const int fin = net.width[l], fout = net.width[l + 1];
-    const R* W = theta + net.w_off[l];
-    const R* b = theta + net.b_off[l];
+    const int fin = PJ_NET_WIDTH(&net, &deep, l), fout = PJ_NET_WIDTH(&net, &deep, l + 1);
+    const R* W = theta + PJ_NET_W_OFF(&net, &deep, l);
+    const R* b = theta + PJ_NET_B_OFF(&net, &deep, l);
     const int tid = threadIdx.x + part * blockDim.x, nt = blockDim.x * nparts;   // this block's share of every loop
     if (l == 0) {
         const int hp1 = pl.hp[n][1];
@@ -282,6 +312,10 @@ static int plan_info_impl(const PjSpec* spec, int64_t n_points, int64_t* out, in
     const long long tail[6] = {pl.tc, pl.tc /* tc_bwd: the reverse kernel always matches the forward kernel */, pl.tp, pl.ws_tcrec, pl.grid_bwd, pl.n_tiles1};
     for (int i = 0; i < 6 && k < n_out; ++i) out[k++] = tail[i];
     for (int n = PJ_MAX_NETS; n < PJ_MAX_NETS_ALL; ++n) per_net(n);   // nets 4..15, after the older layout
+    for (int n = 0; n < PJ_MAX_NETS_ALL; ++n) {   // layers of networks deeper than PJ_MAX_LINEAR, after that
+        for (int l = PJ_MAX_LINEAR + 1; l <= PJ_MAX_LINEAR_ALL && k < n_out; ++l) out[k++] = pl.hp[n][l];
+        for (int l = PJ_MAX_LINEAR; l < PJ_MAX_LINEAR_ALL && k < n_out; ++l) out[k++] = pl.zj_off[n][l];
+    }
     return 0;
 }
 
@@ -291,7 +325,8 @@ static int pack_impl(const PjSpec* spec, const R* theta, R* theta_pack, R* zero_
     PackArgs a;
     copy_spec(a.spec, *spec);
     if (int rc = device_plan<R>(*spec, 1, 0, a.plan)) return rc;
-    pack_kernel<R><<<dim3(spec->n_nets * PJ_MAX_LINEAR, PACK_PARTS), 256, 0, (cudaStream_t)stream>>>(a, theta, theta_pack, zero_buf, n_zero);
+    pack_kernel<R><<<dim3(spec->n_nets * pack_stride(a.spec), PACK_PARTS), 256, 0, (cudaStream_t)stream>>>(a, theta, theta_pack, zero_buf,
+                                                                                                         n_zero);
     return check_cuda(cudaGetLastError(), "pack launch");
 }
 
@@ -355,7 +390,7 @@ static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, con
     typename ArgsOf<R>::K1 a;
     memset(&a, 0, sizeof(a));
     copy_spec(a.spec, *spec);
-    for (int n = 0; n < spec->n_nets && n < PJ_MAX_NETS_ALL; ++n) a.net[n] = *PJ_SPEC_NET(spec, n);
+    for (int n = 0; n < a.spec.n_nets && n < PJ_MAX_NETS_ALL; ++n) a.net[n] = kernel_net(a.spec, n);
     if (spec->wl > 0 && (!prog_w || prog_w_len < 1)) return fail(-1, "spec->wl=%d needs a weight program", spec->wl);
     if (spec->wl == 0) prog_w_len = 0;
     if (int rc = device_plan<R>(*spec, n, prog_len, a.plan, prog_w_len)) return rc;
@@ -470,7 +505,7 @@ static int run_k2(const PjSpec* spec, const R* const* coords, int64_t n_points, 
     typename ArgsOf<R>::K2 a;
     memset(&a, 0, sizeof(a));
     copy_spec(a.spec, *spec);
-    for (int n = 0; n < spec->n_nets && n < PJ_MAX_NETS_ALL; ++n) a.net[n] = *PJ_SPEC_NET(spec, n);
+    for (int n = 0; n < a.spec.n_nets && n < PJ_MAX_NETS_ALL; ++n) a.net[n] = kernel_net(a.spec, n);
     if (int rc = device_plan<R>(*spec, n_points, 0, a.plan)) return rc;
     if (workspace_bytes < (size_t)a.plan.ws_bytes)
         return fail(-1, "workspace too small: %zu < %lld bytes", workspace_bytes, a.plan.ws_bytes);

@@ -55,12 +55,26 @@ enum : int {
     OP_ATAN, OP_ERF, OP_ST_W, OP_POW   // OP_POW: double programs only
 };
 
+// Network instance n as the FFMA kernels index it: PJ_SPEC_NET(&spec, n) with the layers of spec.deep[n] in the same
+// arrays, filled on the host through the PJ_SPEC_* accessors (pinnjet_api.cu).  One flat table keeps the kernels' indexing --
+// and so their register allocation -- what it is for networks of at most PJ_MAX_LINEAR Linear layers.
+struct KNet {
+    int32_t n_in;
+    int32_t in_coord[PJ_MAX_COORDS];
+    int32_t n_linear;
+    int32_t width[PJ_MAX_LINEAR_ALL + 1];
+    int32_t act;
+    int32_t yrow0;
+    int64_t w_off[PJ_MAX_LINEAR_ALL];
+    int64_t b_off[PJ_MAX_LINEAR_ALL];
+};
+
 // Kernel arguments for element type R (float, or double for the PJ_F64 instances of the FFMA kernels).
 template <typename R>
 struct K1ArgsT {
     PjSpec spec;
     Plan plan;
-    PjNet net[PJ_MAX_NETS_ALL];          // PJ_SPEC_NET(&spec, n) for n < spec.n_nets, contiguous: what the FFMA kernels index
+    KNet net[PJ_MAX_NETS_ALL];           // instance n < spec.n_nets, contiguous and with all its layers: what the FFMA kernels index
     const R* coords[PJ_MAX_COORDS];
     const R* pack;
     const int4* prog;
@@ -86,7 +100,7 @@ template <typename R>
 struct K2ArgsT {
     PjSpec spec;
     Plan plan;
-    PjNet net[PJ_MAX_NETS_ALL];          // PJ_SPEC_NET(&spec, n) for n < spec.n_nets, contiguous: what the FFMA kernels index
+    KNet net[PJ_MAX_NETS_ALL];           // instance n < spec.n_nets, contiguous and with all its layers: what the FFMA kernels index
     const R* coords[PJ_MAX_COORDS];
     const R* pack;
     long long N;

@@ -19,7 +19,7 @@ namespace pj {
 // ---- producer warp: stream the hidden->hidden weight matrices of every tile, in consumption order -------------------
 // forward order: net 0..n-1, Linear l = 1..L-1, row chunks ascending.  backward (K2): Linear l = L-1..1.
 template <bool kForward, typename R>
-__device__ __forceinline__ void weight_producer(const PjSpec& sp, const PjNet* nets, const Plan& pl, const R* __restrict__ pack,
+__device__ __forceinline__ void weight_producer(const PjSpec& sp, const KNet* nets, const Plan& pl, const R* __restrict__ pack,
                                                 R* ring, uint64_t* full, uint64_t* empty, int my_tiles) {
     const bool resident = kForward ? pl.resident_fwd : pl.resident_bwd;
     const int n_stage = kForward ? pl.n_stage : pl.n_stage_bwd;
@@ -236,7 +236,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
         }
 
         for (int n = 0; n < sp.n_nets; ++n) {
-            const PjNet& net = A.net[n];
+            const KNet& net = A.net[n];
             const int L = net.n_linear - 1;   // hidden layers
             const int act_kind = net.act;
             R wq[P][WL > 0 ? WL : 1];

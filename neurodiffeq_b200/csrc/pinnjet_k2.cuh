@@ -136,7 +136,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
         const R* seed_tile = A.seeds + tile * ((long long)sp.n_yrows * T);
 
         for (int n = 0; n < sp.n_nets; ++n) {
-            const PjNet& net = A.net[n];
+            const KNet& net = A.net[n];
             const int L = net.n_linear - 1;
             const int act_kind = net.act;
             const int n_out = net.width[net.n_linear];
@@ -471,7 +471,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     // flush the shared-memory gradient accumulators into this CTA's partial (padded units are dropped)
     bar_compute<NTC>();
     for (int n = 0; n < sp.n_nets; ++n) {
-        const PjNet& net = A.net[n];
+        const KNet& net = A.net[n];
         const int L = net.n_linear - 1;
         const int h1 = net.width[1], hL = net.width[L], hpL = pl.hp[n][L], n_out = net.width[net.n_linear];
         auto sgsum = [&](int idx) {

@@ -12,13 +12,14 @@ static int round_up(int v, int m) { return (v + m - 1) / m * m; }
 static long long round_up_ll(long long v, long long m) { return (v + m - 1) / m * m; }
 
 static const PjNet& net_of(const PjSpec& sp, int n) { return *PJ_SPEC_NET(&sp, n); }   // instance n < sp.n_nets
+static int width_of(const PjSpec& sp, int n, int l) { return PJ_SPEC_WIDTH(&sp, n, l); }   // layer l <= n_linear of instance n
+static int outputs_of(const PjSpec& sp, int n) { return width_of(sp, n, net_of(sp, n).n_linear); }
+static bool deep_net(const PjSpec& sp, int n) { return net_of(sp, n).n_linear > PJ_MAX_LINEAR; }
 
 static int max_outputs(const PjSpec& sp) {   // widest output Linear of all nets
     int m = 0;
-    for (int i = 0; i < sp.n_nets; ++i) {
-        const PjNet& net = net_of(sp, i);
-        if (net.width[net.n_linear] > m) m = net.width[net.n_linear];
-    }
+    for (int i = 0; i < sp.n_nets; ++i)
+        if (outputs_of(sp, i) > m) m = outputs_of(sp, i);
     return m;
 }
 
@@ -169,9 +170,11 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     int hmax = 32, yrows = 0;
     for (int n = 0; n < sp.n_nets; ++n) {
         const PjNet& net = net_of(sp, n);
-        if (net.n_linear < 2 || net.n_linear > PJ_MAX_LINEAR) return fail(-1, "net %d: n_linear=%d out of range", n, net.n_linear);
+        if (net.n_linear < 2) return fail(-1, "net %d: n_linear=%d out of range", n, net.n_linear);
+        if (net.n_linear > PJ_MAX_LINEAR_ALL)
+            return fail(-2, "net %d: %d Linear layers (max %d)", n, net.n_linear, PJ_MAX_LINEAR_ALL);
         if (net.n_in < 1 || net.n_in > PJ_MAX_COORDS || net.width[0] != net.n_in) return fail(-1, "net %d: bad n_in", n);
-        const int n_out = net.width[net.n_linear];
+        const int n_out = outputs_of(sp, n);
         if (n_out < 1 || n_out > PJ_MAX_OUT) return fail(-2, "net %d: %d output units (max %d)", n, n_out, PJ_MAX_OUT);
         if (net.act < PJ_ACT_TANH || net.act > PJ_ACT_ELU) return fail(-2, "net %d: unknown activation", n);
         if (net.yrow0 != yrows) return fail(-1, "net %d: yrow0 must be %d", n, yrows);
@@ -181,9 +184,9 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
         for (int i = 0; i < net.n_in; ++i)
             if (net.in_coord[i] < 0 || net.in_coord[i] >= sp.n_coords) return fail(-1, "net %d: bad in_coord", n);
         for (int h = 1; h < net.n_linear; ++h) {
-            if (net.width[h] < 1 || net.width[h] > PJ_MAX_WIDTH)
-                return fail(-2, "net %d: hidden width %d not in 1..%d", n, net.width[h], PJ_MAX_WIDTH);
-            pl.hp[n][h] = round_up(net.width[h], 32);
+            const int w = width_of(sp, n, h);
+            if (w < 1 || w > PJ_MAX_WIDTH) return fail(-2, "net %d: hidden width %d not in 1..%d", n, w, PJ_MAX_WIDTH);
+            pl.hp[n][h] = round_up(w, 32);
             if (pl.hp[n][h] > hmax) hmax = pl.hp[n][h];
         }
     }
@@ -208,7 +211,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     int off = 0;
     for (int n = 0; n < sp.n_nets; ++n) {
         const PjNet& net = net_of(sp, n);
-        const int L = net.n_linear - 1, n_out = net.width[net.n_linear];
+        const int L = net.n_linear - 1, n_out = outputs_of(sp, n);
         pl.s_wt0[n] = off; off += round_up(net.n_in * pl.hp[n][1], 4);
         pl.s_dz[n] = off; off += PJ_MAX_DIRS * pl.hp[n][1];
         for (int l = 0; l < L; ++l) { pl.s_b[n][l] = off; off += pl.hp[n][l + 1]; }
@@ -240,7 +243,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     off = 0;
     for (int n = 0; n < sp.n_nets; ++n) {
         const PjNet& net = net_of(sp, n);
-        const int L = net.n_linear - 1, n_out = net.width[net.n_linear];
+        const int L = net.n_linear - 1, n_out = outputs_of(sp, n);
         pl.g_w0[n] = off; off += pl.hp[n][1] * net.n_in;
         for (int l = 0; l < L; ++l) { pl.g_b[n][l] = off; off += pl.hp[n][l + 1]; }
         pl.g_wl[n] = off; off += n_out * pl.hp[n][L];
@@ -252,13 +255,15 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     // ---- kernel selection ----
     // Tensor-core kernels (pinnjet_tc.cuh): every hidden layer exactly 64 wide (after padding), at most 8 jet channels, at
     // most 4 outputs per net (one 16-byte row of the output Linear), no third-order channels, at most PJ_MAX_NETS network
-    // instances (their register arrays are sized by it), tanh and sine only, the weight images of both kernels resident in
-    // shared memory.  The decision may not depend on the program length (only pj_forward* know it): the programs get a
+    // instances (their register arrays are sized by it) of at most PJ_MAX_LINEAR Linear layers (they read PjNet alone),
+    // tanh and sine only, the weight images of both kernels resident in shared memory.  The decision may not depend on the program length (only pj_forward* know it): the programs get a
     // fixed reserve.
     bool tc = esz == 4 && dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4 && sp.n3 == 0 &&
               sp.n_nets <= PJ_MAX_NETS && !uses_extended_activation(sp);
-    for (int n = 0; tc && n < sp.n_nets; ++n)
-        for (int h = 1; h < net_of(sp, n).n_linear; ++h) tc = tc && pl.hp[n][h] == TC_H;
+    for (int n = 0; tc && n < sp.n_nets; ++n) {
+        tc = !deep_net(sp, n);
+        for (int h = 1; tc && h < net_of(sp, n).n_linear; ++h) tc = pl.hp[n][h] == TC_H;
+    }
     if (tc) {   // both kernels tile like the forward kernel; seeds / weights / records are shared as is
         int n_hidden = 0;
         for (int n = 0; n < sp.n_nets; ++n) n_hidden += net_of(sp, n).n_linear - 1;
@@ -349,8 +354,8 @@ int make_plan(const PjSpec& sp, long long N, int prog_len, int prog_w_len, const
     if (esz != 4 && esz != 8) return fail(-1, "element size %d (4 or 8)", esz);
     int occ = 0, hmax = 0;
     for (int n = 0; n < sp.n_nets && n < PJ_MAX_NETS_ALL; ++n)
-        for (int h = 1; h < net_of(sp, n).n_linear && h <= PJ_MAX_LINEAR; ++h)
-            if (net_of(sp, n).width[h] > hmax) hmax = net_of(sp, n).width[h];
+        for (int h = 1; h < net_of(sp, n).n_linear && h <= PJ_MAX_LINEAR_ALL; ++h)
+            if (width_of(sp, n, h) > hmax) hmax = width_of(sp, n, h);
     Plan narrow;
     int rc128 = -1;
     if (hmax <= 64) {

@@ -72,18 +72,18 @@ struct Plan {
     int T1, P1, Q1, RS1, ntc1, n_tiles1; // K1 tile (a multiple of T): wider thread tile (Q1 = 8) -> fewer smem wavefronts
     int n_tiles, grid, grid_bwd, hmax, ntc;   // grid: K1 CTAs, grid_bwd: K2 CTAs (= gradient partials)
     int n_stage, n_stage_bwd, resident_fwd, resident_bwd, chunks_fwd, chunks_bwd;   // n_stage: forward ring
-    int hp[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR + 1];   // padded widths (hidden -> multiple of 32; input/output unpadded)
+    int hp[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR_ALL + 1];   // padded widths (hidden -> multiple of 32; input/output unpadded)
     // ---- packed parameter copy (float offsets) ----
     int small_floats;
     int s_wt0[PJ_MAX_NETS_ALL];              // [n_in][hp1]       first Linear, K-major
     int s_dz[PJ_MAX_NETS_ALL];               // [PJ_MAX_DIRS][hp1] first-order seeds  W0 . dir_f  (point independent)
-    int s_b[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR]; // hidden biases, padded
+    int s_b[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR_ALL]; // hidden biases, padded
     int s_wlt[PJ_MAX_NETS_ALL];              // [hpL][n_out]      last Linear, K-major        (forward)
     int s_wlo[PJ_MAX_NETS_ALL];              // [n_out][hpL]      last Linear, out-major      (backward)
     int s_bout[PJ_MAX_NETS_ALL];
-    long long b_wt[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR];   // hidden->hidden Linear l: [in_p][out_p]  (forward B operand)
-    long long b_wo[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR];   //                          [out_p][in_p]  (adjoint B operand)
-    long long b_wimg[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR];   // tensor-core path: 3 bf16 split images of W_l, K-major SWIZZLE_128B (float offset)
+    long long b_wt[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR_ALL];   // hidden->hidden Linear l: [in_p][out_p]  (forward B operand)
+    long long b_wo[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR_ALL];   //                          [out_p][in_p]  (adjoint B operand)
+    long long b_wimg[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR_ALL];   // tensor-core path: 3 bf16 split images of W_l, K-major SWIZZLE_128B (float offset)
     long long b_woutimg[PJ_MAX_NETS_ALL];    // tensor-core path: 3 bf16 split images [16 x 64] of the output Linear (rows >= n_out zero)
     int n_out_max;                       // widest output Linear of all nets (K2 instances with > K2_OUT_GROUP differ)
     int tc;                              // 1: K1 and K2 run the hidden-layer GEMMs on wgmma (pinnjet_k1tc3.cuh, pinnjet_k2tc2.cuh)
@@ -93,10 +93,10 @@ struct Plan {
     long long ws_tcrec;                  // workspace offset (bytes) of those records
     long long pack_floats;
     // ---- small-gradient accumulators in shared memory (float offsets) ----
-    int g_w0[PJ_MAX_NETS_ALL], g_b[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR], g_wl[PJ_MAX_NETS_ALL], g_bout[PJ_MAX_NETS_ALL], sgrad_floats;
+    int g_w0[PJ_MAX_NETS_ALL], g_b[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR_ALL], g_wl[PJ_MAX_NETS_ALL], g_bout[PJ_MAX_NETS_ALL], sgrad_floats;
     int sgrad_copies;                    // one private copy per point-group block of warps (no atomics)
     // ---- workspace (byte offsets) ----
-    int zj_off[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR];       // float offset of hidden layer h (1..L) z-jets inside a tile block
+    int zj_off[PJ_MAX_NETS_ALL][PJ_MAX_LINEAR_ALL];       // float offset of hidden layer h (1..L) z-jets inside a tile block
     long long zj_tile_floats;
     long long ws_zj, ws_seed, ws_gpart, ws_loss, ws_bytes;
     // ---- shared memory (byte offsets) ----

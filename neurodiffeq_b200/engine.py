@@ -18,6 +18,7 @@ _LIB_PATH = os.environ.get("PINNJET_LIB", os.path.join(_HERE, "csrc", "libpinnje
 
 PJ_MAX_NETS, PJ_MAX_LINEAR, PJ_MAX_COORDS, PJ_MAX_DIRS = 4, 8, 8, 4
 PJ_MAX_NETS_ALL = 16   # network instances per problem: PjSpec.net holds the first PJ_MAX_NETS, net_more the rest
+PJ_MAX_LINEAR_ALL = 16   # Linear layers per network: PjNet holds the first PJ_MAX_LINEAR, PjSpec.deep the rest
 SUPPORTED_SCHEMES = [(1, 0), (1, 1), (2, 0), (2, 1), (2, 2), (3, 0), (3, 3), (4, 4)]
 COMBINED_SCHEMES = [(2, 2), (3, 3), (4, 4)]   # (n1, n2) that also exist with ONE weighted second-order channel (wl = n2)
 COMBINED_ONLY = [(4, 4)]                      # ... and these exist ONLY in that form (9 separate channels do not fit)
@@ -35,17 +36,39 @@ class PjNet(ctypes.Structure):
                 ("w_off", ctypes.c_int64 * PJ_MAX_LINEAR), ("b_off", ctypes.c_int64 * PJ_MAX_LINEAR)]
 
 
+class PjNetDeep(ctypes.Structure):
+    _fields_ = [("width", ctypes.c_int32 * (PJ_MAX_LINEAR_ALL - PJ_MAX_LINEAR)),
+                ("w_off", ctypes.c_int64 * (PJ_MAX_LINEAR_ALL - PJ_MAX_LINEAR)),
+                ("b_off", ctypes.c_int64 * (PJ_MAX_LINEAR_ALL - PJ_MAX_LINEAR))]
+
+
 class PjSpec(ctypes.Structure):
     _fields_ = [("abi_version", ctypes.c_int32), ("n_coords", ctypes.c_int32), ("n_nets", ctypes.c_int32),
                 ("n1", ctypes.c_int32), ("n2", ctypes.c_int32), ("wl", ctypes.c_int32),
                 ("dir", (ctypes.c_float * PJ_MAX_COORDS) * PJ_MAX_DIRS),
                 ("n_funcs", ctypes.c_int32), ("n_eq", ctypes.c_int32), ("n_yrows", ctypes.c_int32),
                 ("n_slots", ctypes.c_int32), ("n_theta", ctypes.c_int64), ("net", PjNet * PJ_MAX_NETS),
-                ("n3", ctypes.c_int32), ("net_more", PjNet * (PJ_MAX_NETS_ALL - PJ_MAX_NETS))]
+                ("n3", ctypes.c_int32), ("net_more", PjNet * (PJ_MAX_NETS_ALL - PJ_MAX_NETS)),
+                ("deep", PjNetDeep * PJ_MAX_NETS_ALL)]
 
     def net_at(self, n):
         """network instance n: net[n] for the first PJ_MAX_NETS, then net_more (PJ_SPEC_NET of pinnjet.h)"""
         return self.net[n] if n < PJ_MAX_NETS else self.net_more[n - PJ_MAX_NETS]
+
+    def set_layers(self, n, widths, w_off, b_off):
+        """widths (n_linear + 1) and Linear offsets (n_linear) of instance n: the first layers into its PjNet, layers beyond
+        PJ_MAX_LINEAR into deep[n] (PJ_SPEC_WIDTH / PJ_SPEC_W_OFF / PJ_SPEC_B_OFF of pinnjet.h)"""
+        net, deep = self.net_at(n), self.deep[n]
+        for l, w in enumerate(widths):
+            if l <= PJ_MAX_LINEAR:
+                net.width[l] = w
+            else:
+                deep.width[l - PJ_MAX_LINEAR - 1] = w
+        for l, (wo, bo) in enumerate(zip(w_off, b_off)):
+            if l < PJ_MAX_LINEAR:
+                net.w_off[l], net.b_off[l] = wo, bo
+            else:
+                deep.w_off[l - PJ_MAX_LINEAR], deep.b_off[l - PJ_MAX_LINEAR] = wo, bo
 
 
 class PjSizes(ctypes.Structure):
@@ -338,15 +361,12 @@ class FusedProblem:
             for i, c in enumerate(nd.in_coord):
                 net.in_coord[i] = c
             net.n_linear = len(nd.linears)
-            if net.n_linear > PJ_MAX_LINEAR:
-                raise NotImplementedError(f"{net.n_linear} Linear layers (max {PJ_MAX_LINEAR})")
-            for i, w in enumerate(nd.widths):
-                net.width[i] = w
+            if net.n_linear > PJ_MAX_LINEAR_ALL:
+                raise NotImplementedError(f"{net.n_linear} Linear layers (max {PJ_MAX_LINEAR_ALL})")
             net.act = nd.act
             net.yrow0 = tp.yrow0[n]
-            for l, lin in enumerate(nd.linears):
-                net.w_off[l] = self._offset_of[id(lin.weight)]
-                net.b_off[l] = self._offset_of[id(lin.bias)]
+            sp.set_layers(n, nd.widths, [self._offset_of[id(lin.weight)] for lin in nd.linears],
+                          [self._offset_of[id(lin.bias)] for lin in nd.linears])
         self.spec = sp
 
     def _register_program_scalars(self):
@@ -594,6 +614,9 @@ class FusedProblem:
                 raise ValueError("the specialised kernel is float32 only (this problem runs in float64)")
             if self._patch_sets:
                 raise ValueError("the program has trainable immediates (Resnet shortcut)")
+            if any(len(nd.linears) > PJ_MAX_LINEAR for nd in self.tp.nets):
+                raise ValueError(f"a network has more than {PJ_MAX_LINEAR} Linear layers (the tensor-core kernels take at most "
+                                 f"{PJ_MAX_LINEAR})")
             if not self.plan_info(1024)["tc"]:
                 raise ValueError("the network is not on the tensor-core path (hidden width != 64 or PINNJET_TC=0)")
             from .jit import JitKernel
@@ -616,10 +639,12 @@ class FusedProblem:
         return ok
 
     def plan_info(self, n_points):
-        """Tiling plan (diagnostics): dict with T, RS, grid, ... plus padded widths and z-jet offsets of all
-        PJ_MAX_NETS_ALL net slots (pj_plan_info: nets 0-3, six trailing fields, then nets 4-15)."""
+        """Tiling plan (diagnostics): dict with T, RS, grid, ... plus padded widths (hp, PJ_MAX_LINEAR_ALL + 1 per net) and
+        z-jet offsets (zj_off, PJ_MAX_LINEAR_ALL per net) of all PJ_MAX_NETS_ALL net slots (pj_plan_info: nets 0-3, six
+        trailing fields, nets 4-15, then the layers beyond PJ_MAX_LINEAR of nets 0-15)."""
         per_net = 2 * PJ_MAX_LINEAR + 1
-        n = 19 + PJ_MAX_NETS * per_net + 6 + (PJ_MAX_NETS_ALL - PJ_MAX_NETS) * per_net
+        per_deep = 2 * (PJ_MAX_LINEAR_ALL - PJ_MAX_LINEAR)
+        n = 19 + PJ_MAX_NETS * per_net + 6 + (PJ_MAX_NETS_ALL - PJ_MAX_NETS) * per_net + PJ_MAX_NETS_ALL * per_deep
         out = (ctypes.c_int64 * n)()
         with torch.cuda.device(self.device):
             _check(self._fn("pj_plan_info")(ctypes.byref(self.spec), n_points, out, n), "pj_plan_info")
@@ -639,7 +664,12 @@ class FusedProblem:
         k = nets(19, PJ_MAX_NETS)
         for i, name in enumerate(("tc", "tc_bwd", "tc_tile_points", "ws_tcrec", "grid_bwd", "n_tiles_fwd")):
             info[name] = int(out[k + i])
-        nets(k + 6, PJ_MAX_NETS_ALL - PJ_MAX_NETS)
+        k = nets(k + 6, PJ_MAX_NETS_ALL - PJ_MAX_NETS)
+        extra = PJ_MAX_LINEAR_ALL - PJ_MAX_LINEAR
+        for hp, zj in zip(info["hp"], info["zj_off"]):
+            hp.extend(int(out[k + i]) for i in range(extra))
+            zj.extend(int(out[k + extra + i]) for i in range(extra))
+            k += 2 * extra
         return info
 
     # ---- CUDA-graph replay of a whole residual+gradient evaluation -----------------------------------------------------

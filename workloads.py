@@ -502,6 +502,86 @@ def _a4(nd):
                     32768, 3 * _fcnn_flops((1, 32, 32, 1), 2), None)
 
 
+# ----------------------------------------------------------------------------------------------------------------------
+# D1..D4  deep networks: more than 8 Linear layers (up to 16), the depth of the PINN literature's standard networks
+# ----------------------------------------------------------------------------------------------------------------------
+def _d1(nd):
+    """The Burgers problem of Raissi, Perdikaris & Karniadakis (2019): u_t + u u_x - (0.01/pi) u_xx = 0 on [-1, 1] x [0, 1],
+    u(x, 0) = -sin(pi x), zero ends (IBVP1D), on their network of 8 hidden layers of 20 tanh units (9 Linear layers)."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(20,) * 8)]
+
+    def make_conditions():
+        return [nd.IBVP1D(x_min=-1, x_max=1, t_min=0, t_min_val=lambda x: -torch.sin(np.pi * x),
+                          x_min_val=lambda t: 0, x_max_val=lambda t: 0)]
+
+    def diff_eqs(u, x, t):
+        return [nd.diff(u, t) + u * nd.diff(u, x) - NU_BURGERS * nd.diff(u, x, order=2)]
+
+    widths = (2,) + (20,) * 8 + (1,)
+    return Workload("d1_raissi_burgers", "Solver2D", ("x", "t"), ((-1.0, 1.0), (0.0, 1.0)), [(widths, "tanh")], make_nets,
+                    make_conditions, diff_eqs, 1, 32768, _fcnn_flops(widths, 4), None)
+
+
+def _d2(nd):
+    """C2's Laplace problem on 9 hidden layers of 64 tanh units (10 Linear layers): a width the tensor-core kernels take, a
+    depth they do not."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(64,) * 9)]
+
+    def make_conditions():
+        return [nd.DirichletBVP2D(x_min=0, x_min_val=lambda y: torch.sin(np.pi * y), x_max=1, x_max_val=lambda y: 0,
+                                  y_min=0, y_min_val=lambda x: 0, y_max=1, y_max_val=lambda x: 0)]
+
+    def diff_eqs(u, x, y):
+        return [nd.diff(u, x, order=2) + nd.diff(u, y, order=2)]
+
+    widths = (2,) + (64,) * 9 + (1,)
+    return Workload("d2_laplace_deep64", "Solver2D", ("x", "y"), ((0.0, 1.0), (0.0, 1.0)), [(widths, "tanh")], make_nets,
+                    make_conditions, diff_eqs, 1, 32768, _fcnn_flops(widths, 5), None)
+
+
+def _d3(nd):
+    """The depth limit: 15 hidden layers of 32 SiLU units (16 Linear layers) on the third-order ODE
+    u''' + u u'' / 2 = exp(-t), u(0) = u'(0) = 0 (jet_order=3)."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(32,) * 15, actv=torch.nn.SiLU)]
+
+    def make_conditions():
+        return [nd.IVP(t_0=0.0, u_0=0.0, u_0_prime=0.0)]
+
+    def diff_eqs(u, t):
+        return [nd.diff(u, t, order=3) + 0.5 * u * nd.diff(u, t, order=2) - torch.exp(-t)]
+
+    widths = (1,) + (32,) * 15 + (1,)
+    return Workload("d3_third_order_silu16", "Solver1D", ("t",), ((0.0, 2.0),), [(widths, "silu")], make_nets,
+                    make_conditions, diff_eqs, 1, 16384, _fcnn_flops(widths, 4), None)
+
+
+def _d4(nd):
+    """6-function linear chain u_i' = k (u_{i-1} - 2 u_i + u_{i+1}) with zero ends, its networks alternating between 2 hidden
+    layers of 32 tanh units and 12 hidden layers of 24 SinActv units (13 Linear layers): 6 instances, deep ones among the
+    first four and after them."""
+    K, k = 6, 2.0
+    shallow, deep = (1, 32, 32, 1), (1,) + (24,) * 12 + (1,)
+    shapes = [(shallow, "tanh") if i % 2 == 0 else (deep, "sin") for i in range(K)]
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(32, 32)) if i % 2 == 0 else
+                nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(24,) * 12, actv=nd.SinActv) for i in range(K)]
+
+    def make_conditions():
+        return [nd.IVP(t_0=0.0, u_0=math.sin(math.pi * (i + 1) / (K + 1))) for i in range(K)]
+
+    def diff_eqs(*args):
+        u, t = args[:K], args[K]
+        side = lambda j: u[j] if 0 <= j < K else 0.0   # noqa: E731
+        return [nd.diff(u[i], t) - k * (side(i - 1) - 2 * u[i] + side(i + 1)) for i in range(K)]
+
+    return Workload("d4_chain_mixed_depths", "Solver1D", ("t",), ((0.0, 1.0),), shapes, make_nets, make_conditions, diff_eqs,
+                    K, 16384, sum(_fcnn_flops(w, 2) for w, _ in shapes), None)
+
+
 _EXTRA = {
     "x1": lambda nd: _heat(nd, "x1_heat_dirichlet_neumann", "right"),
     "x2": lambda nd: _heat(nd, "x2_heat_neumann_dirichlet", "left"),
@@ -542,6 +622,10 @@ _ACTIVATION = {
 }
 ACTIVATION_NAMES = tuple(_ACTIVATION)
 _BUILDERS.update(_ACTIVATION)
+# networks of more than 8 Linear layers (d3 with jet_order=3); kept out of the tuples above as well
+_DEEP = {"d1": _d1, "d2": _d2, "d3": _d3, "d4": _d4}
+DEEP_NAMES = tuple(_DEEP)
+_BUILDERS.update(_DEEP)
 # workloads whose conditions see only the first coordinate (a network of r alone, as SolverSpherical passes it)
 _RADIAL = ("s1", "s2")
 
