@@ -578,11 +578,11 @@ __device__ __forceinline__ void gemm_rows(typename Pair<R>::type (&acc)[Q][C][P 
     }
 }
 
-// The float adjoint GEMM of the reverse kernel: the same tile and the same FMA order per accumulator as gemm_rows, but
-// every point of the tile is a plain float register.  sm_90 has no packed FP32 FMA, and the 64-bit pairs only cost
-// register moves there (ptxas re-pairs the results at the loop back-edge).  The A and B operands of row k + 1 are loaded
-// before the FFMAs of row k, so the shared-memory latency hides behind them; the last row loads itself again instead of
-// reading past the chunk.
+// The float GEMM of the forward kernel and of the reverse kernel's adjoint: the same tile and the same FMA order per
+// accumulator as gemm_rows, but every point of the tile is a plain float register.  sm_90 has no packed FP32 FMA, and
+// the 64-bit pairs only cost register moves there (ptxas re-pairs the results at the loop back-edge).  The A and B
+// operands of row k + 1 are loaded before the FFMAs of row k, so the shared-memory latency hides behind them; the last
+// row loads itself again instead of reading past the chunk.
 template <int P, int Q, int C>
 __device__ __forceinline__ void gemm_rows(float (&acc)[Q][C][P], const float* __restrict__ a_ptr, int RS, int T,
                                           const float* __restrict__ b_ptr, int ldb, int nrows) {
@@ -635,15 +635,15 @@ __device__ __forceinline__ void gemm_rows(float (&acc)[Q][C][P], const float* __
     }
 }
 
-// Accumulator tile of the reverse kernel's adjoint GEMM: plain floats (gemm_rows above) when SCALAR, point pairs for
-// double.
+// Accumulator tile of the FFMA kernels' GEMMs (the forward GEMM, the reverse kernel's adjoint and weight-gradient GEMMs):
+// plain floats (gemm_rows above) when SCALAR, point pairs for double.
 template <typename R, int P, bool SCALAR>
-struct AdjAcc {
+struct GemmAcc {
     typedef typename Pair<R>::type elem;
     static constexpr int n = P / 2;
 };
 template <int P>
-struct AdjAcc<float, P, true> {
+struct GemmAcc<float, P, true> {
     typedef float elem;
     static constexpr int n = P;
 };

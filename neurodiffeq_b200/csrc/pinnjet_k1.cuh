@@ -6,7 +6,7 @@
 //
 // Per tile of T points a CTA keeps ALL jet channels of one hidden layer in shared memory ([unit][channel][point],
 // row stride RS) and walks the layers: the hidden->hidden contraction for the C channels is one register-tiled
-// FP32 GEMM (FFMA, point pairs) whose B operand (K-major weights) is streamed by a producer warp with bulk
+// FP32 GEMM (FFMA, plain float accumulators) whose B operand (K-major weights) is streamed by a producer warp with bulk
 // TMA through an mbarrier ring (kept resident when all layers fit).  The activation-jet rule runs on the accumulator
 // registers, results go back to shared memory in place.  The raw network-output jets of up to 256 points are
 // collected and the residual program is then interpreted with one point per thread.
@@ -74,7 +74,7 @@ struct RingCursor {
 // XA instances: see record_holds_value.
 template <int P, int N1, int N2, int WL, int N3, bool XA, typename R>
 __device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2 + N3], int act_kind, R* __restrict__ act_row, int T,
-                                            R* __restrict__ rec_row, int T2, const R (&wq)[P][WL > 0 ? WL : 1]) {
+                                            R* __restrict__ rec_row, int T2, const R* __restrict__ wrow) {
     constexpr int C = 1 + N1 + N2 + N3;
     auto store = [](R* dst, const R (&v)[P][C], int c) {
         if constexpr (P == 4)
@@ -82,6 +82,11 @@ __device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2 + N3], int ac
         else
             store2(dst, v[0][c], v[1][c]);
     };
+    R wq[P][WL > 0 ? WL : 1];
+#pragma unroll
+    for (int p = 0; p < P; ++p)
+#pragma unroll
+        for (int dd = 0; dd < (WL > 0 ? WL : 1); ++dd) wq[p][dd] = WL > 0 ? wrow[dd * T + p] : R(0);
     R z0s[P];
 #pragma unroll
     for (int p = 0; p < P; ++p) z0s[p] = zq[p][0];
@@ -107,8 +112,10 @@ __device__ __forceinline__ void finish_unit(R (&zq)[P][1 + N1 + N2 + N3], int ac
 
 template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3, bool XA>
 __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
-    typedef typename Pair<R>::type pair;
     constexpr int C = 1 + N1 + N2 + N3;
+    // plain float accumulators in the hidden->hidden GEMM (gemm_rows), except in the third-order and 7-channel instances:
+    // with plain floats ptxas spills more in those, so they keep the point pairs (as the double instances do)
+    constexpr bool SCALAR_ACC = sizeof(R) == 4 && N3 == 0 && C < 7;
     // service warps after the compute warps: 128-thread CTAs (weights always resident: the producer only issues the initial
     // loads) use ONE warp as producer-then-program warp; 256-thread CTAs have a producer warp and a program warp
     constexpr int N_SVC = NTC == 128 ? 1 : 2;
@@ -198,7 +205,9 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
     // -------------------------------------------- compute warps --------------------------------------------------------
     const JobMap jm(tid, T, P, Q);
     const int p0 = jm.p0, u0 = jm.u0;
-    RingCursor<R> cur{0, pl.n_stage, pl.resident_fwd != 0, full, empty, ring};
+    // 128-thread CTAs always keep every chunk resident (at most MAX_STAGES of them): as compile-time facts, the cursor holds
+    // no stage count or residency flag across the GEMM
+    RingCursor<R> cur{0, NTC == 128 ? MAX_STAGES : pl.n_stage, NTC == 128 || pl.resident_fwd != 0, full, empty, ring};
     const bool train = A.mode == 1;
     int bslot = 0, batch_idx = 0;   // tile slot inside the current batch, batches handed to the program warp so far
     PJ_T_DECL   // slots: 0 setup, 1 layer0, 2 gemm, 3 barrier-after-gemm, 4 epilogue, 5 output layer, 6 program
@@ -239,11 +248,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
             const KNet& net = A.net[n];
             const int L = net.n_linear - 1;   // hidden layers
             const int act_kind = net.act;
-            R wq[P][WL > 0 ? WL : 1];
-#pragma unroll
-            for (int p = 0; p < P; ++p)
-#pragma unroll
-                for (int dd = 0; dd < (WL > 0 ? WL : 1); ++dd) wq[p][dd] = WL > 0 ? wbuf[(n * WL + dd) * T + p0 + p] : 0.0f;
+            const R* wrow = wbuf + n * WL * T + p0;   // per-point weights of this thread's points (WL > 0)
 
             // ---------------- Linear 0: coordinates -> hidden 1 (first-order channels are columns of W) ----------------
             {
@@ -285,7 +290,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
 #pragma unroll
                             for (int s2 = 0; s2 < N2 + N3; ++s2) zq[p][1 + N1 + s2] = 0.0f;   // second and third orders: 0
                         }
-                        finish_unit<P, N1, N2, WL, N3, XA>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
+                        finish_unit<P, N1, N2, WL, N3, XA>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wrow);
                     }
                 }
             }
@@ -296,13 +301,14 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
             for (int l = 1; l < L; ++l) {
                 const int K = pl.hp[n][l], NO = pl.hp[n][l + 1];
                 const bool valid = u0 < NO;
-                pair acc[Q][C][P / 2];
+                typedef GemmAcc<R, P, SCALAR_ACC> GA;
+                typename GA::elem acc[Q][C][GA::n];
 #pragma unroll
                 for (int q = 0; q < Q; ++q)
 #pragma unroll
                     for (int c = 0; c < C; ++c)
 #pragma unroll
-                        for (int h = 0; h < P / 2; ++h) acc[q][c][h] = pair{};
+                        for (int h = 0; h < GA::n; ++h) acc[q][c][h] = typename GA::elem{};
                 const int rpc = chunk_elems(sizeof(R)) / NO;
                 for (int r0 = 0; r0 < K; r0 += rpc) {
                     const R* chunk = cur.acquire();
@@ -324,7 +330,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
                         for (int c = 0; c < C; ++c)
 #pragma unroll
                             for (int p = 0; p < P; ++p) zq[p][c] = pick<P>(acc[q][c], p) + (c == 0 ? bias : 0.0f);
-                        finish_unit<P, N1, N2, WL, N3, XA>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wq);
+                        finish_unit<P, N1, N2, WL, N3, XA>(zq, act_kind, act + u * RS + p0, T, rec ? zrow + u * RS2 : nullptr, T2, wrow);
                     }
                 }
                 bar_compute<NTC>();

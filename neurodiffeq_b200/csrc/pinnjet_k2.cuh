@@ -319,7 +319,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                 }
                 // (2a) a_bar_{h-1} = W_l^T z_bar_h
                 const bool valid = u0 < HK;
-                typedef AdjAcc<R, P, SCALAR_ACC> AA;
+                typedef GemmAcc<R, P, SCALAR_ACC> AA;
                 typename AA::elem acc[Q][C][AA::n];
 #pragma unroll
                 for (int q = 0; q < Q; ++q)
@@ -380,7 +380,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                     R* gw = gpart + net.w_off[l];
                     for (int wt = warp; wt < n_kb * n_jb; wt += N_CWARPS) {
                         const int jb = (wt / n_kb) * 32, kb = (wt % n_kb) * 32;
-                        typedef AdjAcc<R, 2, SCALAR_ACC> WA;   // one point pair per output: two floats or one pair
+                        typedef GemmAcc<R, 2, SCALAR_ACC> WA;   // one point pair per output: two floats or one pair
                         typename WA::elem wacc[WJ][WK][WA::n];
 #pragma unroll
                         for (int i = 0; i < WJ; ++i)

@@ -200,7 +200,8 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     if ((pl.T / pl.P) % 8 != 0 || pl.T > pl.ntc) return fail(-3, "internal: tile %d unsupported", pl.T);
     pl.RS = C * pl.T + row_pad(esz);
     pl.n_tiles = (int)((N + pl.T - 1) / pl.T);
-    // K1: 8 units per thread (half the shared-memory wavefronts per FFMA of the 4-unit tile); its tile is a multiple of T
+    // K1: 8 units per thread for 128-wide nets (half the shared-memory wavefronts per FFMA of the 4-unit tile), 4 for narrow
+    // ones (FFMA_Q, as K2); its tile is a multiple of T
     pl.P1 = pl.P;
     pl.Q1 = hmax > 64 ? FFMA_Q_WIDE : FFMA_Q;   // wide nets are GEMM-bound (fewer smem wavefronts); narrow ones want more CTAs per SM
     const bool k1_ok = set_k1_tile(pl, hmax <= 64 ? 128 : 256, N, esz) ||
