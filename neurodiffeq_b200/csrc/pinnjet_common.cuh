@@ -271,28 +271,29 @@ __device__ __forceinline__ R warp_sum(R v) {
 
 // Reduce-scatter over the 8 point-group lanes (recursive halving): every thread contributes 8 (or 4) partial sums, lane l
 // of each 8-lane group returns the total of value l (value l >> 1 for the 4-value form, in both lanes of a pair):
-// 7 (4) shuffles instead of the 24 (12) of one butterfly all-reduce per value.
-template <typename R>
+// 7 (4) shuffles instead of the 24 (12) of one butterfly all-reduce per value.  S: lane distance of adjacent point groups
+// (JobMap::PG_STEP: 1, or 4 in the tensor-core lane map), pg_lane = the point-group index 0..7.
+template <int S = 1, typename R>
 __device__ __forceinline__ R pg_reduce_scatter8(const R (&v)[8], int pg_lane) {
     const bool b2 = pg_lane & 4, b1 = pg_lane & 2, b0 = pg_lane & 1;
     R w[4], x[2];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
-        w[i] = (b2 ? v[i + 4] : v[i]) + __shfl_xor_sync(0xffffffffu, b2 ? v[i] : v[i + 4], 4);
+        w[i] = (b2 ? v[i + 4] : v[i]) + __shfl_xor_sync(0xffffffffu, b2 ? v[i] : v[i + 4], 4 * S);
 #pragma unroll
     for (int i = 0; i < 2; ++i)
-        x[i] = (b1 ? w[i + 2] : w[i]) + __shfl_xor_sync(0xffffffffu, b1 ? w[i] : w[i + 2], 2);
-    return (b0 ? x[1] : x[0]) + __shfl_xor_sync(0xffffffffu, b0 ? x[0] : x[1], 1);
+        x[i] = (b1 ? w[i + 2] : w[i]) + __shfl_xor_sync(0xffffffffu, b1 ? w[i] : w[i + 2], 2 * S);
+    return (b0 ? x[1] : x[0]) + __shfl_xor_sync(0xffffffffu, b0 ? x[0] : x[1], S);
 }
-template <typename R>
+template <int S = 1, typename R>
 __device__ __forceinline__ R pg_reduce_scatter4(const R (&v)[4], int pg_lane) {
     const bool b2 = pg_lane & 4, b1 = pg_lane & 2;
     R w[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i)
-        w[i] = (b2 ? v[i + 2] : v[i]) + __shfl_xor_sync(0xffffffffu, b2 ? v[i] : v[i + 2], 4);
-    R x = (b1 ? w[1] : w[0]) + __shfl_xor_sync(0xffffffffu, b1 ? w[0] : w[1], 2);
-    return x + __shfl_xor_sync(0xffffffffu, x, 1);   // value index = pg_lane >> 1
+        w[i] = (b2 ? v[i + 2] : v[i]) + __shfl_xor_sync(0xffffffffu, b2 ? v[i] : v[i + 2], 4 * S);
+    R x = (b1 ? w[1] : w[0]) + __shfl_xor_sync(0xffffffffu, b1 ? w[0] : w[1], 2 * S);
+    return x + __shfl_xor_sync(0xffffffffu, x, S);   // value index = pg_lane >> 1
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -635,6 +636,126 @@ __device__ __forceinline__ void gemm_rows(float (&acc)[Q][C][P], const float* __
     }
 }
 
+// ---- TF32 mma.sync with three products per fp32 product (the float GEMMs of the 128-thread narrow instances) -------------
+// x = big + small with big = x rounded to TF32 (nearest, ties away from zero) and small = x - big (exact, |small| <= 2^-11 |x|),
+// which the tensor core reads truncated to TF32; a b ~ a_small b_big + a_big b_small + a_big b_big, each term within ~2^-21
+// |a b|.  The small products go in first: the tensor core truncates each sum into the fp32 accumulator, so the big term is
+// added last.  The rounding takes two integer operations (cvt.rna.tf32.f32 is five on sm_90, most of them for inf / NaN)
+// and matches cvt.rna for finite |x| below 0x1.ffep127 (0x7f7ff000, ~3.4e38); from there up, and for inf, big becomes inf
+// and the products NaN, where an FFMA loop would stay finite up to its own overflow.
+__device__ __forceinline__ void split_tf32(float x, uint32_t& big, uint32_t& small) {
+    big = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
+    small = __float_as_uint(x - __uint_as_float(big));
+}
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+__device__ __forceinline__ void mma_tf32x3(float (&d)[4], const uint32_t (&ab)[4], const uint32_t (&as)[4], const uint32_t (&bb)[2],
+                                           const uint32_t (&bs)[2]) {
+    mma_tf32(d, as, bb);
+    mma_tf32(d, ab, bs);
+    mma_tf32(d, ab, bb);
+}
+
+// Which instances run their float GEMMs on mma.sync: the 128-thread float instances without third-order channels, up to 6
+// channels (the 7-channel (3, 3) scheme keeps the FFMA loops).  The 256-thread ones (one CTA per SM: 128-wide networks)
+// keep the FFMA loops: with two compute warps per SM sub-partition and no other CTA to overlap with, the weight-gradient
+// MMA loop made C3's reverse kernel 3 % slower on an H100.
+template <typename R, int NTC, int C, int N3>
+constexpr bool mma_gemms() { return sizeof(R) == 4 && N3 == 0 && NTC == 128 && C <= 6; }
+
+// gemm_rows on the tensor cores: acc[q][c][p] += sum_k A[k][c][p0+p] * B[k][u0+q] over nrows (a multiple of 8) rows, with
+// the lane map of JobMap<true> (p0 = pw0 + P g, u0 = ub + 4 t for g = lane / 4, t = lane % 4), which is the MMA fragment's:
+//   M rows: m16 tile (c, h), h < P/2: row g <-> point P g + 2h, row g + 8 <-> point P g + 2h + 1 (channel c)
+//   N cols: n8 tile ni < 2: column n <-> unit 4 (n >> 1) + 2 ni + (n & 1), so the C fragment's columns 2t, 2t + 1 are units
+//           4t + 2ni, 4t + 2ni + 1: a thread owns all C channels of its P consecutive points x 4 consecutive units, as in
+//           the FFMA tile, and the epilogues are unchanged.
+//   K:      column t <-> row k0 + 2t, column t + 4 <-> row k0 + 2t + 1.
+// A thread's A operands of a step are one P-float vector per channel and row k0 + 2t, k0 + 2t + 1: with 2 RS = 8 (mod 16)
+// (row_pad), the 64-bit (P = 2) and 128-bit (P = 4) loads of each phase of the warp hit distinct banks.  B is read as
+// single floats; lanes t = 0..3 of one g read one unit from 4 rows, which share a bank (the ring's rows are 64 or 32 floats):
+// 4 of the step's 4 + C P loads conflict 4-way.  AHEAD: step k0 + 8's operands are loaded before step k0's MMAs (K1's
+// instances other than the 2-point ones of up to 4 channels, at their 128-register cap, do without: with it they spill).
+template <int P, int C, bool AHEAD = true>
+__device__ __forceinline__ void gemm_rows_mma(float (&acc)[4][C][P], const float* __restrict__ a_ptr, int RS, int T,
+                                              const float* __restrict__ b_ptr, int ldb, int nrows, int lane) {
+    static_assert(P == 2 || P == 4, "float2 / float4 point rows");
+    const int g = lane >> 2, t = lane & 3;
+    const float* ap = a_ptr + 2 * t * RS;
+    const float* bp = b_ptr - 4 * t + 4 * (g >> 1) + (g & 1) + 2 * t * ldb;
+    struct Ops {
+        float a[2][C][P], b[2][2];   // [row k0 + 2t + i][channel][point], [n-tile][row k0 + 2t + i]
+    };
+    auto load = [&](int k0, Ops& o) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const float* ar = ap + (k0 + i) * RS;
+#pragma unroll
+            for (int c = 0; c < C; ++c) {
+                if constexpr (P == 4) {
+                    const float4 v = *reinterpret_cast<const float4*>(ar + c * T);
+                    o.a[i][c][0] = v.x;
+                    o.a[i][c][1] = v.y;
+                    o.a[i][c][2] = v.z;
+                    o.a[i][c][3] = v.w;
+                } else {
+                    const float2 v = *reinterpret_cast<const float2*>(ar + c * T);
+                    o.a[i][c][0] = v.x;
+                    o.a[i][c][1] = v.y;
+                }
+            }
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni) o.b[ni][i] = bp[(k0 + i) * ldb + 2 * ni];
+        }
+    };
+    if (nrows <= 0) return;
+    float d[C][P / 2][2][4];
+#pragma unroll
+    for (int c = 0; c < C; ++c)
+#pragma unroll
+        for (int h = 0; h < P / 2; ++h)
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) d[c][h][ni][e] = acc[2 * ni + (e & 1)][c][2 * h + (e >> 1)];
+    Ops cur;
+    if constexpr (AHEAD) load(0, cur);
+#pragma unroll 1
+    for (int k0 = 0; k0 < nrows; k0 += 8) {
+        Ops nxt;
+        if constexpr (AHEAD) load(min(k0 + 8, nrows - 8), nxt);   // the last step loads itself again, not past the chunk
+        else load(k0, cur);
+        uint32_t bb[2][2], bs[2][2];
+#pragma unroll
+        for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) split_tf32(cur.b[ni][i], bb[ni][i], bs[ni][i]);
+#pragma unroll
+        for (int c = 0; c < C; ++c)
+#pragma unroll
+            for (int h = 0; h < P / 2; ++h) {
+                uint32_t ab[4], as[4];   // rows g, g + 8 x columns t, t + 4
+                split_tf32(cur.a[0][c][2 * h], ab[0], as[0]);
+                split_tf32(cur.a[0][c][2 * h + 1], ab[1], as[1]);
+                split_tf32(cur.a[1][c][2 * h], ab[2], as[2]);
+                split_tf32(cur.a[1][c][2 * h + 1], ab[3], as[3]);
+#pragma unroll
+                for (int ni = 0; ni < 2; ++ni) mma_tf32x3(d[c][h][ni], ab, as, bb[ni], bs[ni]);
+            }
+        if constexpr (AHEAD) cur = nxt;
+    }
+#pragma unroll
+    for (int c = 0; c < C; ++c)
+#pragma unroll
+        for (int h = 0; h < P / 2; ++h)
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) acc[2 * ni + (e & 1)][c][2 * h + (e >> 1)] = d[c][h][ni][e];
+}
+
 // Accumulator tile of the FFMA kernels' GEMMs (the forward GEMM, the reverse kernel's adjoint and weight-gradient GEMMs):
 // plain floats (gemm_rows above) when SCALAR, point pairs for double.
 template <typename R, int P, bool SCALAR>
@@ -676,15 +797,19 @@ __device__ __forceinline__ float pick(const float (&v)[P], int p) { return v[p];
 #define PJ_T_FLUSH(base)
 #endif
 
-// thread -> (point group, unit group) mapping shared by K1 and K2: a warp covers 8 point groups x 4 unit groups
+// thread -> (point group, unit group) mapping shared by K1 and K2: a warp covers 8 point groups x 4 unit groups.  MMA: the
+// lane map of gemm_rows_mma (point group lane / 4, unit group lane % 4) instead of lane % 8, lane / 8; PG_STEP is the lane
+// distance of adjacent point groups (the stride of pg_reduce_scatter*).
+template <bool MMA = false>
 struct JobMap {
+    static constexpr int PG_STEP = MMA ? 4 : 1;
     int p0, u0, pg_lane;
     __device__ __forceinline__ JobMap(int tid, int T, int P, int Q) {
         const int warp = tid >> 5, lane = tid & 31;
         const int n_pgb = (T / P) >> 3;
-        pg_lane = lane & 7;
+        pg_lane = MMA ? lane >> 2 : lane & 7;
         p0 = P * ((warp % n_pgb) * 8 + pg_lane);
-        u0 = Q * ((warp / n_pgb) * 4 + (lane >> 3));
+        u0 = Q * ((warp / n_pgb) * 4 + (MMA ? lane & 3 : lane >> 3));
     }
 };
 

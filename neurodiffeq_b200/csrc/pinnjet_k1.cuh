@@ -203,7 +203,9 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
     }
 
     // -------------------------------------------- compute warps --------------------------------------------------------
-    const JobMap jm(tid, T, P, Q);
+    // the hidden-layer GEMM on the tensor cores (gemm_rows_mma), with the MMA lane map
+    constexpr bool MMA = mma_gemms<R, NTC, C, N3>();
+    const JobMap<MMA> jm(tid, T, P, Q);
     const int p0 = jm.p0, u0 = jm.u0;
     // 128-thread CTAs always keep every chunk resident (at most MAX_STAGES of them): as compile-time facts, the cursor holds
     // no stage count or residency flag across the GEMM
@@ -312,7 +314,10 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
                 const int rpc = chunk_elems(sizeof(R)) / NO;
                 for (int r0 = 0; r0 < K; r0 += rpc) {
                     const R* chunk = cur.acquire();
-                    if (valid) gemm_rows<P, Q, C>(acc, act + r0 * RS + p0, RS, T, chunk + u0, NO, min(rpc, K - r0));
+                    if (valid) {
+                        if constexpr (MMA) gemm_rows_mma<P, C, P == 2 && C <= 4>(acc, act + r0 * RS + p0, RS, T, chunk + u0, NO, min(rpc, K - r0), lane);
+                        else gemm_rows<P, Q, C>(acc, act + r0 * RS + p0, RS, T, chunk + u0, NO, min(rpc, K - r0));
+                    }
                     cur.release(lane);
                 }
                 PJ_T_MARK(2)

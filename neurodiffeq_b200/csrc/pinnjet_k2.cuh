@@ -3,12 +3,14 @@
 //
 // Inputs per tile: seeds dL/d(raw output jets) and the z-jets of every hidden layer, both written by K1.
 // Per hidden layer h (from the last to the first) a CTA
-//   1. pulls the adjoint of the layer's a-jets through W^T   -- register-tiled FFMA GEMM, out-major weights streamed by
-//      the producer warp with bulk TMA (same ring as K1);
+//   1. pulls the adjoint of the layer's a-jets through W^T   -- register-tiled GEMM (mma_gemms instances: TF32 mma.sync with
+//      three products per fp32 product; the others: FFMA), out-major weights streamed by the producer warp with bulk TMA
+//      (same ring as K1);
 //   2. applies the reverse of the activation-jet rule (needs tanh''' / sin''') on the accumulator registers, re-creating
 //      the a-jets of the layer below from its z-jets (bulk-TMA'd from the workspace) on the way;
-//   3. accumulates the weight gradient  W_bar += z_bar (x) a_prev  over channels and points -- second FFMA GEMM whose
-//      4x4 output tile per thread is added into a per-CTA partial buffer (thread-owned, no atomics);
+//   3. accumulates the weight gradient  W_bar += z_bar (x) a_prev  over channels and points -- second GEMM (on mma.sync
+//      or FFMA, as the first) whose output tile per thread is added
+//      into a per-CTA partial buffer (every element has one owner thread);
 // bias / first-layer / last-layer gradients are reduced over the point lanes with warp shuffles into shared memory.
 // K2b sums the per-CTA partials into grad_theta (+=, like autograd accumulation, solvers.py:360-362).
 #pragma once
@@ -69,6 +71,57 @@ __device__ __forceinline__ auto wgrad_sum(const PairT (&v)[1]) {
 }
 __device__ __forceinline__ float wgrad_sum(const float (&v)[2]) { return v[0] + v[1]; }
 
+// ---- the float weight-gradient GEMM on the tensor cores: mma.sync.m16n8k8 TF32, three products per fp32 product ----------
+// Warp tile out[j][k], j < 32, k < 32: += sum_r G[j][r] * Z[k][r] over the n_r = C*T (channel, point) pairs, as 2 x 4 m16n8
+// tiles (M = j, N = k, K = r).  With g = lane / 4, t = lane % 4, acc[mi][ni][e] is
+//   j = 16 mi + g + 8 (e >> 1),  k = 8 ni + 2 t + (e & 1).
+// Fragment loads are single floats, A at (j = 16 mi + g (+8), r = r0 + t (+4)), B at (k = 8 ni + g, r = r0 + t (+4)): when
+// RS = 4 (mod 8) (row_pad keeps every float row stride so) the 8 rows g RS start in 8 distinct multiples of 4 banks, so a
+// warp's load hits 32 distinct banks.  The fragments of step r0 + 8 are loaded before the MMAs of step r0.
+struct WgradMma {
+    uint32_t a[2][2][4], b[4][2][2];   // [tile][big, small][fragment register]
+    __device__ __forceinline__ void load(const float* __restrict__ g, const float* __restrict__ z, int RS, int r0) {
+        const float* gr = g + r0;
+        const float* zr = z + r0;
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi) {
+            const float* p = gr + 16 * mi * RS;
+            split_tf32(p[0], a[mi][0][0], a[mi][1][0]);
+            split_tf32(p[8 * RS], a[mi][0][1], a[mi][1][1]);
+            split_tf32(p[4], a[mi][0][2], a[mi][1][2]);
+            split_tf32(p[8 * RS + 4], a[mi][0][3], a[mi][1][3]);
+        }
+#pragma unroll
+        for (int ni = 0; ni < 4; ++ni) {
+            const float* p = zr + 8 * ni * RS;
+            split_tf32(p[0], b[ni][0][0], b[ni][1][0]);
+            split_tf32(p[4], b[ni][0][1], b[ni][1][1]);
+        }
+    }
+};
+__device__ __forceinline__ void wgrad_tile_mma(float (&acc)[2][4][4], const float* __restrict__ g_warp,
+                                               const float* __restrict__ z_warp, int RS, int n_r, int lane) {
+    const int g = lane >> 2, t = lane & 3;
+    const float* gb = g_warp + g * RS + t;
+    const float* zb = z_warp + g * RS + t;
+    WgradMma cur;
+    cur.load(gb, zb, RS, 0);
+#pragma unroll 1
+    for (int r0 = 0; r0 < n_r; r0 += 8) {
+        WgradMma nxt;
+        nxt.load(gb, zb, RS, min(r0 + 8, n_r - 8));   // the last step loads itself again instead of reading past the row
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int ni = 0; ni < 4; ++ni) {
+                mma_tf32(acc[mi][ni], cur.a[mi][1], cur.b[ni][0]);
+                mma_tf32(acc[mi][ni], cur.a[mi][0], cur.b[ni][1]);
+                mma_tf32(acc[mi][ni], cur.a[mi][0], cur.b[ni][0]);
+            }
+        cur = nxt;
+    }
+}
+
 // WIDE: some net has more than K2_OUT_GROUP outputs (a separate instance: the <= 4-output code stays as it is).  XA: the
 // extended activation rule (act_x).
 template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE, bool XA>
@@ -77,6 +130,9 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     // plain float accumulators in the adjoint and weight-gradient GEMMs, except in the third-order instances: with them
     // ptxas spills 16 B more in their WIDE instance, so those keep the point pairs (as the double instances do)
     constexpr bool SCALAR_ACC = sizeof(R) == 4 && N3 == 0;
+    // the adjoint and weight-gradient GEMMs on the tensor cores (gemm_rows_mma, wgrad_tile_mma), with the MMA lane map
+    constexpr bool MMA = mma_gemms<R, NTC, C, N3>();
+    constexpr int PGS = JobMap<MMA>::PG_STEP;
     constexpr int NT_COMPUTE = NTC, NT_TOTAL = NTC + 32, N_CWARPS = NTC / 32;
     extern __shared__ __align__(128) unsigned char smem[];
     const PjSpec& sp = A.spec;
@@ -117,7 +173,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
         return;
     }
 
-    const JobMap jm(tid, T, P, Q);
+    const JobMap<MMA> jm(tid, T, P, Q);
     const int p0 = jm.p0, u0 = jm.u0;
     // every (point-group block, unit) pair is owned by exactly one lane -> private accumulation, no atomics
     R* sg = sgrad + (size_t)(warp % ((T / P) >> 3)) * pl.sgrad_floats;
@@ -212,18 +268,18 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                     const int pl8 = jm.pg_lane, i4 = pl8 & 3;
                     {   // reduce over the point lanes: [bias(4) | W_out row 0 (4)], then W_out rows 1.. two at a time
                         const R v0[8] = {gbq[0], gbq[1], gbq[2], gbq[3], gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3]};
-                        const R t0 = pg_reduce_scatter8(v0, pl8);
+                        const R t0 = pg_reduce_scatter8<PGS>(v0, pl8);
                         if (pl8 < 4) sg[pl.g_b[n][L - 1] + u0 + i4] += t0; else sg[pl.g_wl[n] + u0 + i4] += t0;
                         if (n_out > 1) {
                             const R v1[8] = {gwq[1][0], gwq[1][1], gwq[1][2], gwq[1][3],
                                                  gwq[2][0], gwq[2][1], gwq[2][2], gwq[2][3]};
-                            const R t1 = pg_reduce_scatter8(v1, pl8);
+                            const R t1 = pg_reduce_scatter8<PGS>(v1, pl8);
                             if (pl8 < 4) sg[pl.g_wl[n] + hpL + u0 + i4] += t1;
                             else if (n_out > 2) sg[pl.g_wl[n] + 2 * hpL + u0 + i4] += t1;
                         }
                         if (n_out > 3) {
                             const R v2[4] = {gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
-                            const R t2 = pg_reduce_scatter4(v2, pl8);
+                            const R t2 = pg_reduce_scatter4<PGS>(v2, pl8);
                             if (!(pl8 & 1)) sg[pl.g_wl[n] + 3 * hpL + u0 + (pl8 >> 1)] += t2;
                         }
                     }
@@ -259,7 +315,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                         gbq[q] = gb;
                     }
                     const int pl8 = jm.pg_lane, i4 = pl8 & 3;
-                    const R tb = pg_reduce_scatter4(gbq, pl8);
+                    const R tb = pg_reduce_scatter4<PGS>(gbq, pl8);
                     if (!(pl8 & 1)) sg[pl.g_b[n][L - 1] + u0 + (pl8 >> 1)] += tb;
                     for (int o0 = 0; o0 < n_out; o0 += K2_OUT_GROUP) {
                         R gwq[K2_OUT_GROUP][Q];
@@ -288,12 +344,12 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                         const int row = o0 + (pl8 >> 2);   // reduced value pl8: unit u0 + (pl8 & 3) of row o0 (+1 for pl8 >= 4)
                         const R v1[8] = {gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3],
                                              gwq[1][0], gwq[1][1], gwq[1][2], gwq[1][3]};
-                        const R t1 = pg_reduce_scatter8(v1, pl8);
+                        const R t1 = pg_reduce_scatter8<PGS>(v1, pl8);
                         if (row < n_out) sg[pl.g_wl[n] + row * hpL + u0 + i4] += t1;
                         if (o0 + 2 < n_out) {
                             const R v2[8] = {gwq[2][0], gwq[2][1], gwq[2][2], gwq[2][3],
                                                  gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
-                            const R t2 = pg_reduce_scatter8(v2, pl8);
+                            const R t2 = pg_reduce_scatter8<PGS>(v2, pl8);
                             if (row + 2 < n_out) sg[pl.g_wl[n] + (row + 2) * hpL + u0 + i4] += t2;
                         }
                     }
@@ -330,7 +386,10 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                 const int rpc = chunk_elems(sizeof(R)) / HK;
                 for (int r0 = 0; r0 < HJ; r0 += rpc) {
                     const R* chunk = cur.acquire();
-                    if (valid) gemm_rows<P, Q, C>(acc, G + r0 * RS + p0, RS, T, chunk + u0, HK, min(rpc, HJ - r0));
+                    if (valid) {
+                        if constexpr (MMA) gemm_rows_mma<P, C>(acc, G + r0 * RS + p0, RS, T, chunk + u0, HK, min(rpc, HJ - r0), lane);
+                        else gemm_rows<P, Q, C>(acc, G + r0 * RS + p0, RS, T, chunk + u0, HK, min(rpc, HJ - r0));
+                    }
                     cur.release(lane);
                 }
                 PJ_T_MARK(3)
@@ -368,7 +427,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                         }
                         gbq[q] = gb;
                     }
-                    const R tb = pg_reduce_scatter4(gbq, jm.pg_lane);
+                    const R tb = pg_reduce_scatter4<PGS>(gbq, jm.pg_lane);
                     if (!(jm.pg_lane & 1)) sg[pl.g_b[n][h - 2] + u0 + (jm.pg_lane >> 1)] += tb;
                 }
                 bar_compute<NTC>();
@@ -380,25 +439,38 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                     R* gw = gpart + net.w_off[l];
                     for (int wt = warp; wt < n_kb * n_jb; wt += N_CWARPS) {
                         const int jb = (wt / n_kb) * 32, kb = (wt % n_kb) * 32;
-                        typedef GemmAcc<R, 2, SCALAR_ACC> WA;   // one point pair per output: two floats or one pair
-                        typename WA::elem wacc[WJ][WK][WA::n];
-#pragma unroll
-                        for (int i = 0; i < WJ; ++i)
-#pragma unroll
-                            for (int jj = 0; jj < WK; ++jj)
-#pragma unroll
-                                for (int hh = 0; hh < WA::n; ++hh) wacc[i][jj][hh] = typename WA::elem{};
-                        wgrad_tile(wacc, G + (size_t)(jb + jl) * RS, 4, Zb + (size_t)(kb + kl) * RS, 8, RS, C * T);
                         // every output element is owned by one thread of this CTA, so the fire-and-forget reduction
                         // (RED.ADD, no return value to wait for) into the CTA's private partial is race-free and ordered
+                        if constexpr (MMA) {
+                            float wacc[2][4][4] = {};
+                            wgrad_tile_mma(wacc, G + (size_t)jb * RS, Zb + (size_t)kb * RS, RS, C * T, lane);
 #pragma unroll
-                        for (int i = 0; i < WJ; ++i) {
-                            const int j = jb + jl + 4 * i;
+                            for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-                            for (int jj = 0; jj < WK; ++jj) {
-                                const int k = kb + kl + 8 * jj;
-                                if (j < width_j && k < width_k) {
-                                    atomicAdd(&gw[(size_t)j * width_k + k], wgrad_sum(wacc[i][jj]));
+                                for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+                                    for (int e = 0; e < 4; ++e) {
+                                        const int j = jb + 16 * mi + (lane >> 2) + 8 * (e >> 1);
+                                        const int k = kb + 8 * ni + 2 * (lane & 3) + (e & 1);
+                                        if (j < width_j && k < width_k) atomicAdd(&gw[(size_t)j * width_k + k], wacc[mi][ni][e]);
+                                    }
+                        } else {
+                            typedef GemmAcc<R, 2, SCALAR_ACC> WA;   // one point pair per output: two floats or one pair
+                            typename WA::elem wacc[WJ][WK][WA::n];
+#pragma unroll
+                            for (int i = 0; i < WJ; ++i)
+#pragma unroll
+                                for (int jj = 0; jj < WK; ++jj)
+#pragma unroll
+                                    for (int hh = 0; hh < WA::n; ++hh) wacc[i][jj][hh] = typename WA::elem{};
+                            wgrad_tile(wacc, G + (size_t)(jb + jl) * RS, 4, Zb + (size_t)(kb + kl) * RS, 8, RS, C * T);
+#pragma unroll
+                            for (int i = 0; i < WJ; ++i) {
+                                const int j = jb + jl + 4 * i;
+#pragma unroll
+                                for (int jj = 0; jj < WK; ++jj) {
+                                    const int k = kb + kl + 8 * jj;
+                                    if (j < width_j && k < width_k) atomicAdd(&gw[(size_t)j * width_k + k], wgrad_sum(wacc[i][jj]));
                                 }
                             }
                         }
@@ -452,11 +524,11 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                         }
                         if (net.n_in <= 4) {
                             const R v4[4] = {sv[0], sv[1], sv[2], sv[3]};
-                            const R t = pg_reduce_scatter4(v4, jm.pg_lane);
+                            const R t = pg_reduce_scatter4<PGS>(v4, jm.pg_lane);
                             const int i = jm.pg_lane >> 1;
                             if (!(jm.pg_lane & 1) && i < net.n_in) sg[pl.g_w0[n] + u * net.n_in + i] += t;
                         } else {
-                            const R t = pg_reduce_scatter8(sv, jm.pg_lane);
+                            const R t = pg_reduce_scatter8<PGS>(sv, jm.pg_lane);
                             if (jm.pg_lane < net.n_in) sg[pl.g_w0[n] + u * net.n_in + jm.pg_lane] += t;
                         }
                     }
