@@ -295,6 +295,14 @@ __device__ __forceinline__ R pg_reduce_scatter4(const R (&v)[4], int pg_lane) {
     R x = (b1 ? w[1] : w[0]) + __shfl_xor_sync(0xffffffffu, b1 ? w[0] : w[1], 2 * S);
     return x + __shfl_xor_sync(0xffffffffu, x, S);   // value index = pg_lane >> 1
 }
+// 2-value form: value pg_lane >> 2, in all four lanes of a quad (3 shuffles)
+template <int S = 1, typename R>
+__device__ __forceinline__ R pg_reduce_scatter2(const R (&v)[2], int pg_lane) {
+    const bool b2 = pg_lane & 4;
+    R x = (b2 ? v[1] : v[0]) + __shfl_xor_sync(0xffffffffu, b2 ? v[0] : v[1], 4 * S);
+    x += __shfl_xor_sync(0xffffffffu, x, 2 * S);
+    return x + __shfl_xor_sync(0xffffffffu, x, S);
+}
 
 // ---------------------------------------------------------------------------------------------------------------------
 // activation jets (SURVEY.md Appendix A).  Channels: 0 value | 1..N1 first order | N1+1..N1+N2 pure second order |
@@ -665,6 +673,9 @@ __device__ __forceinline__ void mma_tf32x3(float (&d)[4], const uint32_t (&ab)[4
 // MMA loop made C3's reverse kernel 3 % slower on an H100.
 template <typename R, int NTC, int C, int N3>
 constexpr bool mma_gemms() { return sizeof(R) == 4 && N3 == 0 && NTC == 128 && C <= 6; }
+// block size of the reverse kernel instance: the mma_gemms ones run eight compute warps and no producer warp
+template <typename R, int NTC, int C, int N3>
+constexpr int k2_block_threads() { return ffma_k2_threads(NTC, mma_gemms<R, NTC, C, N3>()); }
 
 // gemm_rows on the tensor cores: acc[q][c][p] += sum_k A[k][c][p0+p] * B[k][u0+q] over nrows (a multiple of 8) rows, with
 // the lane map of JobMap<true> (p0 = pw0 + P g, u0 = ub + 4 t for g = lane / 4, t = lane % 4), which is the MMA fragment's:
@@ -678,15 +689,19 @@ constexpr bool mma_gemms() { return sizeof(R) == 4 && N3 == 0 && NTC == 128 && C
 // single floats; lanes t = 0..3 of one g read one unit from 4 rows, which share a bank (the ring's rows are 64 or 32 floats):
 // 4 of the step's 4 + C P loads conflict 4-way.  AHEAD: step k0 + 8's operands are loaded before step k0's MMAs (K1's
 // instances other than the 2-point ones of up to 4 channels, at their 128-register cap, do without: with it they spill).
-template <int P, int C, bool AHEAD = true>
-__device__ __forceinline__ void gemm_rows_mma(float (&acc)[4][C][P], const float* __restrict__ a_ptr, int RS, int T,
+// Q = 2 (the reverse kernel's eight-warp instances): one n8 tile, column n <-> unit ub + n (u0 = ub + 2t), so a thread owns
+// all C channels of its P points x 2 consecutive units.  Its B loads are 2 per step instead of 4, still 4-way conflicts.
+template <int P, int C, bool AHEAD = true, int Q = 4>
+__device__ __forceinline__ void gemm_rows_mma(float (&acc)[Q][C][P], const float* __restrict__ a_ptr, int RS, int T,
                                               const float* __restrict__ b_ptr, int ldb, int nrows, int lane) {
     static_assert(P == 2 || P == 4, "float2 / float4 point rows");
+    static_assert(Q == 2 || Q == 4, "one or two n8 tiles");
+    constexpr int NI = Q / 2;
     const int g = lane >> 2, t = lane & 3;
     const float* ap = a_ptr + 2 * t * RS;
-    const float* bp = b_ptr - 4 * t + 4 * (g >> 1) + (g & 1) + 2 * t * ldb;
+    const float* bp = Q == 4 ? b_ptr - 4 * t + 4 * (g >> 1) + (g & 1) + 2 * t * ldb : b_ptr - 2 * t + g + 2 * t * ldb;
     struct Ops {
-        float a[2][C][P], b[2][2];   // [row k0 + 2t + i][channel][point], [n-tile][row k0 + 2t + i]
+        float a[2][C][P], b[NI][2];   // [row k0 + 2t + i][channel][point], [n-tile][row k0 + 2t + i]
     };
     auto load = [&](int k0, Ops& o) {
 #pragma unroll
@@ -707,17 +722,17 @@ __device__ __forceinline__ void gemm_rows_mma(float (&acc)[4][C][P], const float
                 }
             }
 #pragma unroll
-            for (int ni = 0; ni < 2; ++ni) o.b[ni][i] = bp[(k0 + i) * ldb + 2 * ni];
+            for (int ni = 0; ni < NI; ++ni) o.b[ni][i] = bp[(k0 + i) * ldb + 2 * ni];
         }
     };
     if (nrows <= 0) return;
-    float d[C][P / 2][2][4];
+    float d[C][P / 2][NI][4];
 #pragma unroll
     for (int c = 0; c < C; ++c)
 #pragma unroll
         for (int h = 0; h < P / 2; ++h)
 #pragma unroll
-            for (int ni = 0; ni < 2; ++ni)
+            for (int ni = 0; ni < NI; ++ni)
 #pragma unroll
                 for (int e = 0; e < 4; ++e) d[c][h][ni][e] = acc[2 * ni + (e & 1)][c][2 * h + (e >> 1)];
     Ops cur;
@@ -727,9 +742,9 @@ __device__ __forceinline__ void gemm_rows_mma(float (&acc)[4][C][P], const float
         Ops nxt;
         if constexpr (AHEAD) load(min(k0 + 8, nrows - 8), nxt);   // the last step loads itself again, not past the chunk
         else load(k0, cur);
-        uint32_t bb[2][2], bs[2][2];
+        uint32_t bb[NI][2], bs[NI][2];
 #pragma unroll
-        for (int ni = 0; ni < 2; ++ni)
+        for (int ni = 0; ni < NI; ++ni)
 #pragma unroll
             for (int i = 0; i < 2; ++i) split_tf32(cur.b[ni][i], bb[ni][i], bs[ni][i]);
 #pragma unroll
@@ -742,7 +757,7 @@ __device__ __forceinline__ void gemm_rows_mma(float (&acc)[4][C][P], const float
                 split_tf32(cur.a[1][c][2 * h], ab[2], as[2]);
                 split_tf32(cur.a[1][c][2 * h + 1], ab[3], as[3]);
 #pragma unroll
-                for (int ni = 0; ni < 2; ++ni) mma_tf32x3(d[c][h][ni], ab, as, bb[ni], bs[ni]);
+                for (int ni = 0; ni < NI; ++ni) mma_tf32x3(d[c][h][ni], ab, as, bb[ni], bs[ni]);
             }
         if constexpr (AHEAD) cur = nxt;
     }
@@ -751,7 +766,7 @@ __device__ __forceinline__ void gemm_rows_mma(float (&acc)[4][C][P], const float
 #pragma unroll
         for (int h = 0; h < P / 2; ++h)
 #pragma unroll
-            for (int ni = 0; ni < 2; ++ni)
+            for (int ni = 0; ni < NI; ++ni)
 #pragma unroll
                 for (int e = 0; e < 4; ++e) acc[2 * ni + (e & 1)][c][2 * h + (e >> 1)] = d[c][h][ni][e];
 }

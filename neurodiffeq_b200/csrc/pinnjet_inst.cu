@@ -94,17 +94,21 @@ cudaError_t launch_reduce_f64(const double* gpart, int n_parts, long long n_thet
 #if PJ_F64
 typedef K1ArgsF64 K1A;
 typedef K2ArgsF64 K2A;
+typedef double KR;
 constexpr int kEsz = 8;
 // the double instances are tuned for one CTA per SM in both kernels: their accumulators take twice the registers
 constexpr int kMinB1_128 = 1, kMinB2_128 = 1;
 #else
 typedef K1Args K1A;
 typedef K2Args K2A;
+typedef float KR;
 constexpr int kEsz = 4;
 // CTAs per SM the register allocation is tuned for (shared memory may allow fewer): 128-thread CTAs share an SM
 constexpr int kMinB1_128 = 3, kMinB2_128 = 2;
 #endif
 constexpr int kP = ffma_tile_points(1 + PJ_N1 + PJ_N2 + PJ_N3, kEsz);
+// block size of the 128-thread reverse kernel: eight compute warps and no producer warp where the GEMMs run on mma.sync
+constexpr int kK2Threads128 = k2_block_threads<KR, 128, 1 + PJ_N1 + PJ_N2 + PJ_N3, PJ_N3>();
 
 // The kernel instance a plan selects and its block size.  `ready`: result of raising the instance's dynamic
 // shared-memory limit, done once per instance.
@@ -147,14 +151,14 @@ static Variant<K2A> k2_variant(const Plan& pl) {
 #endif
     if (pl.n_out_max > K2_OUT_GROUP) {
         if (pl.ntc == 128) {
-            static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, true>, ffma_k2_threads(128));
+            static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, true>, kK2Threads128);
             return v;
         }
         static const auto v = variant(PJ_K2_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, true>, ffma_k2_threads(256));
         return v;
     }
     if (pl.ntc == 128) {
-        static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, false>, ffma_k2_threads(128));
+        static const auto v = variant(PJ_K2_KERNEL<128, kMinB2_128, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, false>, kK2Threads128);
         return v;
     }
     static const auto v = variant(PJ_K2_KERNEL<256, 1, kP, FFMA_Q, PJ_N1, PJ_N2, PJ_WL, PJ_N3, false>, ffma_k2_threads(256));

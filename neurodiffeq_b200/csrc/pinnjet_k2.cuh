@@ -4,8 +4,8 @@
 // Inputs per tile: seeds dL/d(raw output jets) and the z-jets of every hidden layer, both written by K1.
 // Per hidden layer h (from the last to the first) a CTA
 //   1. pulls the adjoint of the layer's a-jets through W^T   -- register-tiled GEMM (mma_gemms instances: TF32 mma.sync with
-//      three products per fp32 product; the others: FFMA), out-major weights streamed by the producer warp with bulk TMA
-//      (same ring as K1);
+//      three products per fp32 product; the others: FFMA), out-major weights streamed with bulk TMA (same ring as K1) by
+//      the producer warp, or in the mma_gemms instances (eight compute warps, no producer warp) by thread 0;
 //   2. applies the reverse of the activation-jet rule (needs tanh''' / sin''') on the accumulator registers, re-creating
 //      the a-jets of the layer below from its z-jets (bulk-TMA'd from the workspace) on the way;
 //   3. accumulates the weight gradient  W_bar += z_bar (x) a_prev  over channels and points -- second GEMM (on mma.sync
@@ -72,14 +72,16 @@ __device__ __forceinline__ auto wgrad_sum(const PairT (&v)[1]) {
 __device__ __forceinline__ float wgrad_sum(const float (&v)[2]) { return v[0] + v[1]; }
 
 // ---- the float weight-gradient GEMM on the tensor cores: mma.sync.m16n8k8 TF32, three products per fp32 product ----------
-// Warp tile out[j][k], j < 32, k < 32: += sum_r G[j][r] * Z[k][r] over the n_r = C*T (channel, point) pairs, as 2 x 4 m16n8
-// tiles (M = j, N = k, K = r).  With g = lane / 4, t = lane % 4, acc[mi][ni][e] is
+// Warp tile out[j][k], j < 32, k < 8 NI: += sum_r G[j][r] * Z[k][r] over the n_r = C*T (channel, point) pairs, as 2 x NI
+// m16n8 tiles (M = j, N = k, K = r; NI = 4: 32 x 32, NI = 2: the 32 x 16 tile of the eight-warp instances).  With
+// g = lane / 4, t = lane % 4, acc[mi][ni][e] is
 //   j = 16 mi + g + 8 (e >> 1),  k = 8 ni + 2 t + (e & 1).
 // Fragment loads are single floats, A at (j = 16 mi + g (+8), r = r0 + t (+4)), B at (k = 8 ni + g, r = r0 + t (+4)): when
 // RS = 4 (mod 8) (row_pad keeps every float row stride so) the 8 rows g RS start in 8 distinct multiples of 4 banks, so a
 // warp's load hits 32 distinct banks.  The fragments of step r0 + 8 are loaded before the MMAs of step r0.
+template <int NI>
 struct WgradMma {
-    uint32_t a[2][2][4], b[4][2][2];   // [tile][big, small][fragment register]
+    uint32_t a[2][2][4], b[NI][2][2];   // [tile][big, small][fragment register]
     __device__ __forceinline__ void load(const float* __restrict__ g, const float* __restrict__ z, int RS, int r0) {
         const float* gr = g + r0;
         const float* zr = z + r0;
@@ -92,28 +94,29 @@ struct WgradMma {
             split_tf32(p[8 * RS + 4], a[mi][0][3], a[mi][1][3]);
         }
 #pragma unroll
-        for (int ni = 0; ni < 4; ++ni) {
+        for (int ni = 0; ni < NI; ++ni) {
             const float* p = zr + 8 * ni * RS;
             split_tf32(p[0], b[ni][0][0], b[ni][1][0]);
             split_tf32(p[4], b[ni][0][1], b[ni][1][1]);
         }
     }
 };
-__device__ __forceinline__ void wgrad_tile_mma(float (&acc)[2][4][4], const float* __restrict__ g_warp,
+template <int NI>
+__device__ __forceinline__ void wgrad_tile_mma(float (&acc)[2][NI][4], const float* __restrict__ g_warp,
                                                const float* __restrict__ z_warp, int RS, int n_r, int lane) {
     const int g = lane >> 2, t = lane & 3;
     const float* gb = g_warp + g * RS + t;
     const float* zb = z_warp + g * RS + t;
-    WgradMma cur;
+    WgradMma<NI> cur;
     cur.load(gb, zb, RS, 0);
 #pragma unroll 1
     for (int r0 = 0; r0 < n_r; r0 += 8) {
-        WgradMma nxt;
+        WgradMma<NI> nxt;
         nxt.load(gb, zb, RS, min(r0 + 8, n_r - 8));   // the last step loads itself again instead of reading past the row
 #pragma unroll
         for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-            for (int ni = 0; ni < 4; ++ni) {
+            for (int ni = 0; ni < NI; ++ni) {
                 mma_tf32(acc[mi][ni], cur.a[mi][1], cur.b[ni][0]);
                 mma_tf32(acc[mi][ni], cur.a[mi][0], cur.b[ni][1]);
                 mma_tf32(acc[mi][ni], cur.a[mi][0], cur.b[ni][0]);
@@ -122,9 +125,31 @@ __device__ __forceinline__ void wgrad_tile_mma(float (&acc)[2][4][4], const floa
     }
 }
 
+// The eight-warp instances have no producer warp: thread 0 issues chunk i of the sequence weight_producer<false> walks (net
+// 0..n-1, Linear l = L-1..1, wrapping into the next tile) into stage i % n_stage_bwd.  Every hidden->hidden matrix of these
+// plans is at most 64 x 64 floats, one chunk (k2_backward_body asserts it), so chunk i of a tile is its i-th matrix.
+template <typename R>
+__device__ __forceinline__ void feed_weight_chunk(const PjSpec& sp, const KNet* nets, const Plan& pl, const R* __restrict__ pack,
+                                                  R* ring, uint64_t* full, int i) {
+    int j = i % pl.chunks_bwd;
+    for (int n = 0; n < sp.n_nets; ++n) {
+        const int nm = nets[n].n_linear - 2;   // hidden->hidden matrices of net n
+        if (j < nm) {
+            const int l = nm - j;
+            const int stage = i % pl.n_stage_bwd;
+            const uint32_t bytes = (uint32_t)(pl.hp[n][l + 1] * pl.hp[n][l]) * (uint32_t)sizeof(R);
+            mbar_arrive_expect_tx(&full[stage], bytes);
+            tma_bulk_g2s(ring + (size_t)stage * chunk_elems(sizeof(R)), pack + pl.b_wo[n][l], bytes, &full[stage]);
+            return;
+        }
+        j -= nm;
+    }
+}
+
 // WIDE: some net has more than K2_OUT_GROUP outputs (a separate instance: the <= 4-output code stays as it is).  XA: the
 // extended activation rule (act_x).
-template <typename R, int NTC, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE, bool XA>
+// QP: units of the plan's thread tile.
+template <typename R, int NTC, int P, int QP, int N1, int N2, int WL, int N3, bool WIDE, bool XA>
 __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     constexpr int C = 1 + N1 + N2 + N3;
     // plain float accumulators in the adjoint and weight-gradient GEMMs, except in the third-order instances: with them
@@ -133,7 +158,14 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     // the adjoint and weight-gradient GEMMs on the tensor cores (gemm_rows_mma, wgrad_tile_mma), with the MMA lane map
     constexpr bool MMA = mma_gemms<R, NTC, C, N3>();
     constexpr int PGS = JobMap<MMA>::PG_STEP;
-    constexpr int NT_COMPUTE = NTC, NT_TOTAL = NTC + 32, N_CWARPS = NTC / 32;
+    // The MMA instances run two compute threads per thread tile of the plan (all C channels of P points x 2 units each):
+    // 2 NTC compute threads, eight warps for NTC = 128, and no producer warp (thread 0 issues the weight chunks,
+    // feed_weight_chunk).  The tile, the shared-memory image and the grid are the plan's.
+    constexpr int Q = MMA ? QP / 2 : QP;
+    constexpr int NT_COMPUTE = MMA ? 2 * NTC : NTC, NT_TOTAL = ffma_k2_threads(NTC, MMA), N_CWARPS = NT_COMPUTE / 32;
+    static_assert(!MMA || (QP == 4 && 64 * 64 * sizeof(R) <= CHUNK_BYTES),
+                  "the weight feed takes every hidden->hidden matrix (at most 64 x 64 for 128-thread plans) as one chunk, so "
+                  "one adjoint GEMM never waits on a chunk that only its own barrier would free");
     extern __shared__ __align__(128) unsigned char smem[];
     const PjSpec& sp = A.spec;
     const Plan& pl = A.plan;
@@ -156,7 +188,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     if (tid == 0) {
         for (int s = 0; s < MAX_STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], N_CWARPS);
+            if constexpr (!MMA) mbar_init(&empty[s], N_CWARPS);
         }
         mbar_init(zfull, 1);
         fence_barrier_init();
@@ -168,7 +200,12 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     for (long long i = tid; i < sp.n_theta; i += NT_TOTAL) gpart[i] = 0.0f;
     __syncthreads();
 
-    if (warp == N_CWARPS) {
+    // weight chunks this CTA loads: those of one tile when they stay resident, else those of all its tiles
+    const int feed_total = my_tiles > 0 ? (pl.resident_bwd ? pl.chunks_bwd : my_tiles * pl.chunks_bwd) : 0;
+    if constexpr (MMA) {
+        if (tid == 0)
+            for (int i = 0; i < min(pl.n_stage_bwd, feed_total); ++i) feed_weight_chunk(sp, A.net, pl, A.pack, ring, full, i);
+    } else if (warp == N_CWARPS) {
         if (lane == 0) weight_producer<false>(sp, A.net, pl, A.pack, ring, full, empty, my_tiles);
         return;
     }
@@ -212,7 +249,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                 tma_bulk_g2s(Zb, zj_tile + pl.zj_off[n][L], bytes, zfull);
             }
             for (int e = tid; e < n_out * C * T; e += NT_COMPUTE) ybar[e] = __ldg(seed_tile + net.yrow0 * T + e);
-            bar_compute<NTC>();
+            bar_compute<NT_COMPUTE>();
             mbar_wait(zfull, zphase);
             zphase ^= 1u;
             PJ_T_MARK(1)
@@ -224,7 +261,6 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
             {
                 const R* wlo = small + pl.s_wlo[n];
                 if constexpr (!WIDE) if (u0 < hpL) {
-                    static_assert(Q == 4, "the gradient reductions below assume 4 units per thread");
                     static_assert(K2_OUT_GROUP == PJ_MAX_NETS, "the first group's reduction below is written for 4 outputs");
                     R gbq[Q], gwq[K2_OUT_GROUP][Q];   // per-thread partials: bias of hidden L, W_out rows of one group
 #pragma unroll
@@ -266,7 +302,21 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                         for (int o = 0; o < K2_OUT_GROUP; ++o) gwq[o][q] = gw[o];
                     }
                     const int pl8 = jm.pg_lane, i4 = pl8 & 3;
-                    {   // reduce over the point lanes: [bias(4) | W_out row 0 (4)], then W_out rows 1.. two at a time
+                    if constexpr (Q == 2) {
+                        // reduce over the point lanes: [bias (2) | W_out rows 0, 1, 2 (2 each)]: value pl8 is unit u0 + (pl8 & 1)
+                        // of the bias (pl8 < 2) or of row (pl8 >> 1) - 1; then row 3 alone
+                        const R v0[8] = {gbq[0], gbq[1], gwq[0][0], gwq[0][1], gwq[1][0], gwq[1][1], gwq[2][0], gwq[2][1]};
+                        const R t0 = pg_reduce_scatter8<PGS>(v0, pl8);
+                        const int row = (pl8 >> 1) - 1, u = u0 + (pl8 & 1);
+                        if (row < 0) sg[pl.g_b[n][L - 1] + u] += t0;
+                        else if (row < n_out) sg[pl.g_wl[n] + row * hpL + u] += t0;
+                        if (n_out > 3) {
+                            const R v2[2] = {gwq[3][0], gwq[3][1]};
+                            const R t2 = pg_reduce_scatter2<PGS>(v2, pl8);
+                            if (!(pl8 & 3)) sg[pl.g_wl[n] + 3 * hpL + u0 + (pl8 >> 2)] += t2;
+                        }
+                    } else {   // reduce over the point lanes: [bias(4) | W_out row 0 (4)], then W_out rows 1.. two at a time
+                        static_assert(Q == 4, "the gradient reductions below assume 4 units per thread");
                         const R v0[8] = {gbq[0], gbq[1], gbq[2], gbq[3], gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3]};
                         const R t0 = pg_reduce_scatter8<PGS>(v0, pl8);
                         if (pl8 < 4) sg[pl.g_b[n][L - 1] + u0 + i4] += t0; else sg[pl.g_wl[n] + u0 + i4] += t0;
@@ -315,8 +365,13 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                         gbq[q] = gb;
                     }
                     const int pl8 = jm.pg_lane, i4 = pl8 & 3;
-                    const R tb = pg_reduce_scatter4<PGS>(gbq, pl8);
-                    if (!(pl8 & 1)) sg[pl.g_b[n][L - 1] + u0 + (pl8 >> 1)] += tb;
+                    if constexpr (Q == 2) {
+                        const R tb = pg_reduce_scatter2<PGS>(gbq, pl8);
+                        if (!(pl8 & 3)) sg[pl.g_b[n][L - 1] + u0 + (pl8 >> 2)] += tb;
+                    } else {
+                        const R tb = pg_reduce_scatter4<PGS>(gbq, pl8);
+                        if (!(pl8 & 1)) sg[pl.g_b[n][L - 1] + u0 + (pl8 >> 1)] += tb;
+                    }
                     for (int o0 = 0; o0 < n_out; o0 += K2_OUT_GROUP) {
                         R gwq[K2_OUT_GROUP][Q];
 #pragma unroll
@@ -341,16 +396,23 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
 #pragma unroll
                             for (int o = 0; o < K2_OUT_GROUP; ++o) gwq[o][q] = gw[o];
                         }
-                        const int row = o0 + (pl8 >> 2);   // reduced value pl8: unit u0 + (pl8 & 3) of row o0 (+1 for pl8 >= 4)
-                        const R v1[8] = {gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3],
-                                             gwq[1][0], gwq[1][1], gwq[1][2], gwq[1][3]};
-                        const R t1 = pg_reduce_scatter8<PGS>(v1, pl8);
-                        if (row < n_out) sg[pl.g_wl[n] + row * hpL + u0 + i4] += t1;
-                        if (o0 + 2 < n_out) {
-                            const R v2[8] = {gwq[2][0], gwq[2][1], gwq[2][2], gwq[2][3],
-                                                 gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
-                            const R t2 = pg_reduce_scatter8<PGS>(v2, pl8);
-                            if (row + 2 < n_out) sg[pl.g_wl[n] + (row + 2) * hpL + u0 + i4] += t2;
+                        if constexpr (Q == 2) {   // reduced value pl8: unit u0 + (pl8 & 1) of row o0 + (pl8 >> 1)
+                            const int row = o0 + (pl8 >> 1);
+                            const R v1[8] = {gwq[0][0], gwq[0][1], gwq[1][0], gwq[1][1], gwq[2][0], gwq[2][1], gwq[3][0], gwq[3][1]};
+                            const R t1 = pg_reduce_scatter8<PGS>(v1, pl8);
+                            if (row < n_out) sg[pl.g_wl[n] + row * hpL + u0 + (pl8 & 1)] += t1;
+                        } else {
+                            const int row = o0 + (pl8 >> 2);   // reduced value pl8: unit u0 + (pl8 & 3) of row o0 (+1 for pl8 >= 4)
+                            const R v1[8] = {gwq[0][0], gwq[0][1], gwq[0][2], gwq[0][3],
+                                                 gwq[1][0], gwq[1][1], gwq[1][2], gwq[1][3]};
+                            const R t1 = pg_reduce_scatter8<PGS>(v1, pl8);
+                            if (row < n_out) sg[pl.g_wl[n] + row * hpL + u0 + i4] += t1;
+                            if (o0 + 2 < n_out) {
+                                const R v2[8] = {gwq[2][0], gwq[2][1], gwq[2][2], gwq[2][3],
+                                                     gwq[3][0], gwq[3][1], gwq[3][2], gwq[3][3]};
+                                const R t2 = pg_reduce_scatter8<PGS>(v2, pl8);
+                                if (row + 2 < n_out) sg[pl.g_wl[n] + (row + 2) * hpL + u0 + i4] += t2;
+                            }
                         }
                     }
                 }
@@ -360,7 +422,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                     sgrad[pl.g_bout[n] + tid] += s;
                 }
             }
-            bar_compute<NTC>();
+            bar_compute<NT_COMPUTE>();
             PJ_T_MARK(2)
 
             // (2) hidden layers h = L .. 2: Linear l = h-1 maps hidden h-1 -> hidden h
@@ -383,14 +445,17 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                     for (int c = 0; c < C; ++c)
 #pragma unroll
                         for (int hh = 0; hh < AA::n; ++hh) acc[q][c][hh] = typename AA::elem{};
-                const int rpc = chunk_elems(sizeof(R)) / HK;
-                for (int r0 = 0; r0 < HJ; r0 += rpc) {
+                if constexpr (MMA) {   // the whole matrix is one chunk
                     const R* chunk = cur.acquire();
-                    if (valid) {
-                        if constexpr (MMA) gemm_rows_mma<P, C>(acc, G + r0 * RS + p0, RS, T, chunk + u0, HK, min(rpc, HJ - r0), lane);
-                        else gemm_rows<P, Q, C>(acc, G + r0 * RS + p0, RS, T, chunk + u0, HK, min(rpc, HJ - r0));
+                    if (valid) gemm_rows_mma<P, C, true, Q>(acc, G + p0, RS, T, chunk + u0, HK, HJ, lane);
+                    ++cur.it;
+                } else {
+                    const int rpc = chunk_elems(sizeof(R)) / HK;
+                    for (int r0 = 0; r0 < HJ; r0 += rpc) {
+                        const R* chunk = cur.acquire();
+                        if (valid) gemm_rows<P, Q, C>(acc, G + r0 * RS + p0, RS, T, chunk + u0, HK, min(rpc, HJ - r0));
+                        cur.release(lane);
                     }
-                    cur.release(lane);
                 }
                 PJ_T_MARK(3)
                 mbar_wait(zfull, zphase);
@@ -427,27 +492,40 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                         }
                         gbq[q] = gb;
                     }
-                    const R tb = pg_reduce_scatter4<PGS>(gbq, jm.pg_lane);
-                    if (!(jm.pg_lane & 1)) sg[pl.g_b[n][h - 2] + u0 + (jm.pg_lane >> 1)] += tb;
+                    if constexpr (Q == 2) {
+                        const R tb = pg_reduce_scatter2<PGS>(gbq, jm.pg_lane);
+                        if (!(jm.pg_lane & 3)) sg[pl.g_b[n][h - 2] + u0 + (jm.pg_lane >> 2)] += tb;
+                    } else {
+                        const R tb = pg_reduce_scatter4<PGS>(gbq, jm.pg_lane);
+                        if (!(jm.pg_lane & 1)) sg[pl.g_b[n][h - 2] + u0 + (jm.pg_lane >> 1)] += tb;
+                    }
                 }
-                bar_compute<NTC>();
+                bar_compute<NT_COMPUTE>();
+                // every thread is done with the chunk this layer's adjoint GEMM read: refill its stage with the chunk
+                // n_stage_bwd ahead (behind the fence, as the record loads)
+                if constexpr (MMA)
+                    if (tid == 0 && !cur.resident && cur.it - 1 + pl.n_stage_bwd < feed_total) {
+                        fence_proxy_async();
+                        feed_weight_chunk(sp, A.net, pl, A.pack, ring, full, cur.it - 1 + pl.n_stage_bwd);
+                    }
                 PJ_T_MARK(5)
                 // (2c) W_l gradient: out[j][k] += sum_{c,pt} G[j][c,pt] * Zb[k][c,pt]
                 {
                     const int width_j = net.width[h], width_k = net.width[h - 1];   // unpadded
-                    const int n_kb = HK / 32, n_jb = HJ / 32;   // warp tile = 32 rows j x 32 rows k
+                    constexpr int WTK = MMA ? 8 * Q : 32;
+                    const int n_kb = HK / WTK, n_jb = HJ / 32;   // warp tile = 32 rows j x WTK rows k
                     R* gw = gpart + net.w_off[l];
                     for (int wt = warp; wt < n_kb * n_jb; wt += N_CWARPS) {
-                        const int jb = (wt / n_kb) * 32, kb = (wt % n_kb) * 32;
+                        const int jb = (wt / n_kb) * 32, kb = (wt % n_kb) * WTK;
                         // every output element is owned by one thread of this CTA, so the fire-and-forget reduction
                         // (RED.ADD, no return value to wait for) into the CTA's private partial is race-free and ordered
                         if constexpr (MMA) {
-                            float wacc[2][4][4] = {};
+                            float wacc[2][WTK / 8][4] = {};
                             wgrad_tile_mma(wacc, G + (size_t)jb * RS, Zb + (size_t)kb * RS, RS, C * T, lane);
 #pragma unroll
                             for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-                                for (int ni = 0; ni < 4; ++ni)
+                                for (int ni = 0; ni < WTK / 8; ++ni)
 #pragma unroll
                                     for (int e = 0; e < 4; ++e) {
                                         const int j = jb + 16 * mi + (lane >> 2) + 8 * (e >> 1);
@@ -476,7 +554,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                         }
                     }
                 }
-                bar_compute<NTC>();
+                bar_compute<NT_COMPUTE>();
                 PJ_T_MARK(6)
                 R* t = G;
                 G = G2;
@@ -534,14 +612,14 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
                     }
                 }
             }
-            bar_compute<NTC>();
+            bar_compute<NT_COMPUTE>();
             PJ_T_MARK(7)
         }
     }
     PJ_T_FLUSH(16)
 
     // flush the shared-memory gradient accumulators into this CTA's partial (padded units are dropped)
-    bar_compute<NTC>();
+    bar_compute<NT_COMPUTE>();
     for (int n = 0; n < sp.n_nets; ++n) {
         const KNet& net = A.net[n];
         const int L = net.n_linear - 1;
@@ -565,7 +643,7 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
 // The float and double kernels: one body (element type R); the float instance keeps its name and argument type.  The
 // _xact kernels carry the extended activation rule (as in pinnjet_k1.cuh).
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
-__global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
+__global__ void __launch_bounds__((k2_block_threads<float, NTC, 1 + N1 + N2 + N3, N3>()), MINB) k2_backward_kernel(const __grid_constant__ K2Args A) {
     k2_backward_body<float, NTC, P, Q, N1, N2, WL, N3, WIDE, false>(A);
 }
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
@@ -573,7 +651,7 @@ __global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel
     k2_backward_body<double, NTC, P, Q, N1, N2, WL, N3, WIDE, false>(A);
 }
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>
-__global__ void __launch_bounds__(ffma_k2_threads(NTC), MINB) k2_backward_kernel_xact(const __grid_constant__ K2Args A) {
+__global__ void __launch_bounds__((k2_block_threads<float, NTC, 1 + N1 + N2 + N3, N3>()), MINB) k2_backward_kernel_xact(const __grid_constant__ K2Args A) {
     k2_backward_body<float, NTC, P, Q, N1, N2, WL, N3, WIDE, true>(A);
 }
 template <int NTC, int MINB, int P, int Q, int N1, int N2, int WL, int N3, bool WIDE>

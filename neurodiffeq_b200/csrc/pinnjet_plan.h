@@ -28,9 +28,11 @@ constexpr int FFMA_Q = 4, FFMA_Q_WIDE = 8;
 // K2 reduces the output-Linear gradient in groups of this many outputs (pinnjet_k2.cuh)
 constexpr int K2_OUT_GROUP = 4;
 // block = compute threads + service warps.  K1: 128-thread CTAs share one producer / program warp, 256-thread CTAs have
-// one of each; K2: one producer warp.
+// one of each; K2: one producer warp.  K2 instances with `eight_warps` (the 128-thread float instances with mma.sync GEMMs,
+// mma_gemms in pinnjet_common.cuh) run two compute threads per thread tile of the plan and no producer warp: a block of
+// 2 * ntc compute threads, on the plan's tile and shared-memory image.
 constexpr int ffma_k1_threads(int ntc) { return ntc + (ntc == 128 ? 32 : 64); }
-constexpr int ffma_k2_threads(int ntc) { return ntc + 32; }
+constexpr int ffma_k2_threads(int ntc, bool eight_warps = false) { return eight_warps ? 2 * ntc : ntc + 32; }
 
 // ---- tensor-core kernels (pinnjet_tc.cuh, pinnjet_k1tc3.cuh, pinnjet_k2tc2.cuh) ----
 constexpr int TC_ROWS = 128;             // GEMM rows per tile
