@@ -44,6 +44,7 @@ extern "C" {
 #define PJ_MAX_COORDS 8
 #define PJ_MAX_DIRS 4     /* first-order jet directions */
 #define PJ_MAX_WIDTH 128  /* hidden width */
+#define PJ_MAX_COEF 32    /* trainable equation coefficients per problem (PjSpec.n_coef) */
 #define PJ_ACT_TANH 0
 #define PJ_ACT_SIN 1
 #define PJ_ACT_SIGMOID 2  /* torch.nn.Sigmoid; this and the two below run on the FFMA kernels only           */
@@ -90,6 +91,12 @@ typedef struct PjSpec {
     int32_t n3;                         /* pure third-order channels of the first n3 directions, after the    */
                                         /* n2 channels (n3 <= n2, wl == 0); 0: none.  Appended last, so a     */
                                         /* zero-initialised spec of an older caller means what it meant       */
+    int32_t n_coef;                     /* trainable equation coefficients: the last n_coef floats of theta   */
+                                        /* (0..PJ_MAX_COEF; 0: none).  The programs' OP_ST_COT k adds to the  */
+                                        /* gradient of theta[n_theta - n_coef + k].  It takes the four bytes  */
+                                        /* of padding after n3, so the struct's size and every other offset   */
+                                        /* stay as they were, and a zero-initialised spec of an older caller  */
+                                        /* has no coefficients                                                */
     PjNet net_more[PJ_MAX_NETS_ALL - PJ_MAX_NETS];   /* instances 4..n_nets-1.  Read only when n_nets > 4, so a  */
                                         /* caller whose struct ends at n3 keeps working with up to 4 nets     */
     PjNetDeep deep[PJ_MAX_NETS_ALL];    /* layers 9..16 of instance n (n_linear > PJ_MAX_LINEAR).  Read only  */
@@ -159,7 +166,10 @@ int pj_forward(const PjSpec* spec, const int32_t* prog_eval /*device*/, int32_t 
  * If rbar != NULL it is float[R][N], the external cotangents the program's OP_RBAR instructions index: n_eq rows of
  * dL/dr supplied by the caller (custom loss_fn, solvers.py:216-226), optionally followed by n_funcs rows of dL/du for
  * losses that also look at the functions; the program must be the matching external-cotangent variant.
- * resid_out may be NULL.  *sumsq_out += sum r^2.                                                              */
+ * resid_out may be NULL.  *sumsq_out += sum r^2.
+ * With spec->n_coef > 0 the program's OP_ST_COT instructions give the per-point cotangents dL/d(coefficient); the
+ * kernel sums them over the points in a fixed order into the workspace, and the following pj_backward adds the sums to
+ * the coefficients' entries of grad_theta (the last n_coef).                                                  */
 int pj_forward_train(const PjSpec* spec, const int32_t* prog_train /*device*/, int32_t prog_len,
                      const int32_t* prog_w /*device or NULL*/, int32_t prog_w_len,
                      const float* const* coords, int64_t n_points, const float* theta_pack,

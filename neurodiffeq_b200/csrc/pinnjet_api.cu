@@ -420,6 +420,10 @@ static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, con
     a.zj = mode == 1 ? reinterpret_cast<R*>(w + (a.plan.tc ? a.plan.ws_tcrec : a.plan.ws_zj)) : nullptr;
     a.seeds = mode == 1 ? reinterpret_cast<R*>(w + a.plan.ws_seed) : nullptr;
     a.wts = mode == 1 ? reinterpret_cast<R*>(w + a.plan.ws_wts) : nullptr;
+    if (mode == 1 && a.spec.n_coef > 0) {
+        a.coef_part = reinterpret_cast<R*>(w + a.plan.ws_coef);
+        a.coef_sum = a.coef_part + (size_t)a.spec.n_coef * max_loss_parts(sizeof(R));
+    }
     const SchemeEntry* e = find_scheme(*spec);
     if (jit_function) {   // the problem's own forward kernel: same arguments, same plan
         if (!a.plan.tc) return fail(-2, "the specialised forward kernel exists for the tensor-core path only");
@@ -519,6 +523,7 @@ static int run_k2(const PjSpec* spec, const R* const* coords, int64_t n_points, 
     a.gpart = reinterpret_cast<R*>(w + a.plan.ws_gpart);
     a.wts = reinterpret_cast<const R*>(w + a.plan.ws_wts);
     a.dbg = reinterpret_cast<float*>(w + a.plan.ws_loss) + LOSS_DBG_WORD;
+    if (a.spec.n_coef > 0) a.coef_sum = reinterpret_cast<const R*>(w + a.plan.ws_coef) + (size_t)a.spec.n_coef * max_loss_parts(sizeof(R));
     const SchemeEntry* e = find_scheme(*spec);
     if (int rc = check_cuda(e->of<R>(uses_extended_activation(*spec)).k2(a, a.plan.grid_bwd, a.plan.k2_bytes, (cudaStream_t)stream),
                             "backward launch"))

@@ -52,7 +52,8 @@ inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, 
 enum : int {
     OP_CONST = 0, OP_COORD, OP_NET, OP_RBAR, OP_PARAM, OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_NEG, OP_SIN, OP_COS, OP_EXP,
     OP_LOG, OP_TANH, OP_SQRT, OP_ABS, OP_SIGN, OP_POWC, OP_RCP, OP_ST_U, OP_ST_R, OP_ST_SEED, OP_TAN, OP_SINH, OP_COSH,
-    OP_ATAN, OP_ERF, OP_ST_W, OP_POW   // OP_POW: double programs only
+    OP_ATAN, OP_ERF, OP_ST_W, OP_POW,  // OP_POW: double programs only
+    OP_ST_COT                          // per-point cotangent of a trainable coefficient (train programs)
 };
 
 // Network instance n as the FFMA kernels index it: PJ_SPEC_NET(&spec, n) with the layers of spec.deep[n] in the same
@@ -94,6 +95,8 @@ struct K1ArgsT {
     float* dbg;                          // diagnostic builds only (PJ_TIMING): phase cycle counters
     R* sumsq_out;                        // non-null: the LAST warp to deliver its partial folds them all into *sumsq_out (+=)
     unsigned* ticket;                    // ... found by this counter (zero between launches; lives in the loss-partial block)
+    R* coef_part;                        // train mode, spec.n_coef > 0: per-CTA cotangent sums [n_coef][max_loss_parts]
+    R* coef_sum;                         // ... and their totals [n_coef], written by the same last warp (read by K2)
 };
 
 template <typename R>
@@ -109,6 +112,7 @@ struct K2ArgsT {
     const R* wts;
     R* gpart;
     float* dbg;
+    const R* coef_sum;                   // spec.n_coef > 0: the forward kernel's coefficient gradients -> CTA 0's partial
 };
 struct K1Args : K1ArgsT<float> {};
 struct K2Args : K2ArgsT<float> {};
@@ -134,9 +138,13 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // that draws the last ticket adds ALL partials to *sumsq_out and re-arms the counter.  Fixed summation order, so the result
 // is run-to-run reproducible: lane l sums partials l, l + 32, l + 64, ... in that order, then the 32 lane sums are combined
 // by an xor-shuffle tree (offsets 16, 8, 4, 2, 1).  Called by whole warps after lane 0 has written part[my index].
+// With n_coef > 0 the same warp also folds the per-CTA coefficient sums coef_part[k * coef_stride + p] (the same order) into
+// coef_sum[k] (=, the totals of this launch).
 template <typename R>
-__device__ __forceinline__ void fold_loss_partials(const R* part, unsigned n_parts, R* sumsq_out, unsigned* ticket, int lane) {
-    if (sumsq_out == nullptr) return;
+__device__ __forceinline__ void fold_loss_partials(const R* part, unsigned n_parts, R* sumsq_out, unsigned* ticket, int lane,
+                                                   const R* coef_part = nullptr, R* coef_sum = nullptr, int n_coef = 0,
+                                                   int coef_stride = 0) {
+    if (sumsq_out == nullptr && n_coef == 0) return;
     unsigned last = 0;
     if (lane == 0) {
         __threadfence();                                   // my partial is visible before my ticket
@@ -149,8 +157,15 @@ __device__ __forceinline__ void fold_loss_partials(const R* part, unsigned n_par
     for (unsigned p = lane; p < n_parts; p += 32) s += __ldcg(part + p);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    for (int k = 0; k < n_coef; ++k) {
+        R c = 0.0f;
+        for (unsigned p = lane; p < n_parts; p += 32) c += __ldcg(coef_part + (size_t)k * coef_stride + p);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+        if (lane == 0) coef_sum[k] = c;
+    }
     if (lane == 0) {
-        *sumsq_out += s;
+        if (sumsq_out) *sumsq_out += s;
         *ticket = 0u;
     }
 }

@@ -172,6 +172,10 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
     if (warp == N_CWARPS + N_SVC - 1) {   // ---------------- program warp: residual program of batch b while the compute warps
         //                                             already work on the tiles of batch b+1 ----------------
         const bool train_pw = A.mode == 1;
+        // trainable coefficients: this lane's sums of the per-point cotangents, [n_coef][32] in shared memory
+        const int n_coef = train_pw ? sp.n_coef : 0;
+        R* cot = n_coef > 0 ? reinterpret_cast<R*>(smem + pl.k1_cot) + lane : nullptr;
+        for (int k = 0; k < n_coef; ++k) cot[k * 32] = 0.0f;
         R my_sumsq = 0.0f;
         const int n_batches = (my_tiles + tiles_per_batch - 1) / tiles_per_batch;
         for (int b = 0; b < n_batches; ++b) {
@@ -188,6 +192,8 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
                                        ? A.seeds + (gidx / T2) * ((long long)sp.n_yrows * T2) + (gidx % T2) : nullptr;
                 if (gidx < A.N) {
                     ProgIOT<R> io{A.coords, gidx, A.N, yb + bp, EB, A.rbar, A.loss_scale, A.u_out, A.r_out, seed_tile, T2};
+                    io.cot = cot;
+                    io.n_cot = n_coef;
                     my_sumsq += run_program<32>(prog_s, A.prog_len, slots + lane, io);
                 } else if (seed_tile) {
                     for (int r = 0; r < sp.n_yrows; ++r) seed_tile[r * T2] = 0.0f;   // padded points: zero adjoint
@@ -198,7 +204,12 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
         }
         my_sumsq = warp_sum(my_sumsq);
         if (lane == 0) A.loss_part[blockIdx.x] = my_sumsq;
-        fold_loss_partials(A.loss_part, gridDim.x, A.sumsq_out, A.ticket, lane);
+        for (int k = 0; k < n_coef; ++k) {   // this CTA's sum of each coefficient's cotangents, beside the loss partial
+            const R c = warp_sum(cot[k * 32]);
+            if (lane == 0) A.coef_part[k * max_loss_parts(sizeof(R)) + blockIdx.x] = c;
+        }
+        fold_loss_partials(A.loss_part, gridDim.x, A.sumsq_out, A.ticket, lane, A.coef_part, A.coef_sum, n_coef,
+                           max_loss_parts(sizeof(R)));
         return;
     }
 

@@ -197,7 +197,10 @@ __device__ __forceinline__ void k2_backward_body(const K2ArgsT<R>& A) {
     pdl_wait();                       // the forward kernel (records, seeds) and, before it, K0 have completed
     for (int i = tid; i < pl.small_floats; i += NT_TOTAL) small[i] = __ldg(A.pack + i);
     for (int i = tid; i < pl.sgrad_floats * pl.sgrad_copies; i += NT_TOTAL) sgrad[i] = 0.0f;
-    for (long long i = tid; i < sp.n_theta; i += NT_TOTAL) gpart[i] = 0.0f;
+    for (long long i = tid; i < sp.n_theta - sp.n_coef; i += NT_TOTAL) gpart[i] = 0.0f;
+    // trainable coefficients (the last n_coef parameters): their gradients, summed by the forward kernel, are CTA 0's
+    // partial, so that the reduction adds them to grad_theta with every other parameter
+    for (int k = tid; k < sp.n_coef; k += NT_TOTAL) gpart[sp.n_theta - sp.n_coef + k] = blockIdx.x == 0 ? A.coef_sum[k] : R(0);
     __syncthreads();
 
     // weight chunks this CTA loads: those of one tile when they stay resident, else those of all its tiles

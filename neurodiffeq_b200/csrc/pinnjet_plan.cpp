@@ -50,6 +50,7 @@ int k1_ffma_layout(const PjSpec& sp, Plan& pl, int n_stage, int prog_len, int pr
     img.place(pl.k1_wslots, "wslots", sp.wl > 0 ? sp.n_slots * pl.ntc1 * esz : 0);
     img.place(pl.k1_prog, "prog", prog_len * 16);
     img.place(pl.k1_progw, "progw", prog_w_len * 16);
+    if (sp.n_coef > 0) img.place(pl.k1_cot, "cot", sp.n_coef * 32 * esz);
     if (regions) *regions = img;
     return img.bytes;
 }
@@ -163,6 +164,8 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     // a third-order channel needs the first and second channel of its direction; the combined channel has no pure seconds
     if (sp.n3 < 0 || sp.n3 > sp.n2 || (sp.n3 > 0 && sp.wl != 0))
         return fail(-1, "inconsistent n3=%d (n2=%d, wl=%d)", sp.n3, sp.n2, sp.wl);
+    if (sp.n_coef < 0 || sp.n_coef > sp.n_theta) return fail(-1, "n_coef=%d out of range (n_theta=%lld)", sp.n_coef, (long long)sp.n_theta);
+    if (sp.n_coef > PJ_MAX_COEF) return fail(-2, "%d trainable coefficients (max %d)", sp.n_coef, PJ_MAX_COEF);
     const int C = 1 + sp.n1 + sp.n2 + sp.n3;
     pl.C = C;
     pl.P = ffma_tile_points(C, esz);
@@ -260,7 +263,7 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     // tanh and sine only, the weight images of both kernels resident in shared memory.  The decision may not depend on the program length (only pj_forward* know it): the programs get a
     // fixed reserve.
     bool tc = esz == 4 && dev.tc_level > 0 && C <= 8 && hmax == TC_H && pl.n_out_max <= 4 && sp.n3 == 0 &&
-              sp.n_nets <= PJ_MAX_NETS && !uses_extended_activation(sp);
+              sp.n_nets <= PJ_MAX_NETS && !uses_extended_activation(sp) && sp.n_coef == 0;
     for (int n = 0; tc && n < sp.n_nets; ++n) {
         tc = !deep_net(sp, n);
         for (int h = 1; tc && h < net_of(sp, n).n_linear; ++h) tc = pl.hp[n][h] == TC_H;
@@ -344,6 +347,10 @@ static int plan_for_ntc(const PjSpec& sp, long long N, int prog_len, int prog_w_
     pl.ws_wts = round_up_ll(pl.ws_gpart + e * sp.n_theta * pl.grid_bwd, 256);
     pl.ws_tcrec = round_up_ll(pl.ws_wts + e * sp.n_nets * sp.wl * pl.T * pl.n_tiles, 256);
     pl.ws_bytes = round_up_ll(pl.ws_tcrec + (pl.tc ? 4ll * pl.tc_rec_tile_floats * pl.n_tiles1 : 0ll), 256);
+    if (sp.n_coef > 0) {   // sized by the largest forward grid, which only pj_forward* know exactly (it depends on the program)
+        pl.ws_coef = pl.ws_bytes;
+        pl.ws_bytes = round_up_ll(pl.ws_coef + e * sp.n_coef * (max_loss_parts(esz) + 1), 256);
+    }
     return 0;
 }
 

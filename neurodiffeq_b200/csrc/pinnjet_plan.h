@@ -106,6 +106,9 @@ struct Plan {
     int k1_wbuf, k1_wslots, k1_progw;    // combined second-order channel: per-point weights, their interpreter state
     long long ws_wts;                    // workspace: weights [tile][n_nets*wl][T] for K2
     int k2_g0, k2_g1, k2_zb, k2_ring, k2_small, k2_ybar, k2_sgrad, k2_misc, k2_bytes;
+    // ---- trainable coefficients (spec.n_coef > 0 only; FFMA kernels) ----
+    int k1_cot;                          // K1 shared memory: the program warp's per-lane cotangent sums [n_coef][32]
+    long long ws_coef;                   // workspace: per-CTA sums [n_coef][max_loss_parts(esz)], then the totals [n_coef]
 };
 
 // One kernel's shared-memory image, built region after region: each placement sets a Plan offset field; the list of

@@ -26,6 +26,8 @@ struct ProgIOT {
     int T;
     R* w_out = nullptr;           // weight program: OP_ST_W row -> w_out[row * w_stride]
     int w_stride = 0;
+    R* cot = nullptr;             // train programs with coefficients: OP_ST_COT k adds to cot[k * 32] (this lane's sums),
+    int n_cot = 0;                // ... for 0 <= k < n_cot (spec.n_coef); other indices are ignored
 };
 using ProgIO = ProgIOT<float>;
 
@@ -57,6 +59,9 @@ __device__ __forceinline__ R run_program(const int4* __restrict__ prog, int len,
             }
         } else if (op == OP_ST_W) {
             io.w_out[ins.y * io.w_stride] = slot[ins.z * SLOT_STRIDE];
+            continue;
+        } else if (op == OP_ST_COT) {
+            if ((unsigned)ins.y < (unsigned)io.n_cot) io.cot[ins.y * 32] += slot[ins.z * SLOT_STRIDE];
             continue;
         } else if (op >= OP_ST_U && op <= OP_ST_SEED) {
             const R a = slot[ins.z * SLOT_STRIDE];

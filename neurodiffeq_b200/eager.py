@@ -57,6 +57,7 @@ class EagerProblem:
 
     # ---- parameters: the same flat [theta], [grad | sum r^2] buffers as the fused engine ------------------------------
     def _adopt_parameters(self):
+        """theta = [network parameters | trainable tensors of the equations and conditions], as in the fused engine."""
         params, seen = [], set()
         for m in self.nets:
             m.to(device=self.device, dtype=self.dtype)
@@ -64,6 +65,9 @@ class EagerProblem:
                 if id(p) not in seen:
                     seen.add(id(p))
                     params.append(p)
+        coefs = self._coefficient_leaves(seen)
+        params += coefs
+        self.n_coef = sum(t.numel() for t in coefs)   # the last n_coef entries of theta, as in the fused engine
         n_theta = sum(p.numel() for p in params)
         self.theta = torch.empty(n_theta, dtype=self.dtype, device=self.device)
         self.gradbuf = torch.zeros(n_theta + 1, dtype=self.dtype, device=self.device)
@@ -78,6 +82,36 @@ class EagerProblem:
                 self.offsets.append(off)
                 off += n
         self.n_theta = n_theta
+
+    def _coefficient_leaves(self, seen):
+        """Trainable tensors other than the network parameters that the functions and residuals depend on (equation
+        coefficients, also those the user transforms, such as ``torch.exp(log_k)``): the leaves of a probe evaluation's
+        autograd graph, in the order a depth-first walk from the residuals meets them.  Leaves the evaluation creates itself
+        (the reference's ``torch.ones_like(x, requires_grad=True)`` boundary abscissae) differ between two probes and are
+        not parameters."""
+        second = {id(t) for t in self._graph_leaves(seen)}
+        return [t for t in self._graph_leaves(seen) if id(t) in second]
+
+    def _graph_leaves(self, seen):
+        probe = [torch.linspace(0.25, 0.75, 2, dtype=self.dtype, device=self.device) * (1.0 + 0.1 * i)
+                 for i in range(self.n_coords)]
+        cols = self._columns(probe)
+        funcs, res, aux = self._evaluate(probe, cols=cols)
+        seen = seen | {id(c) for c in cols}
+        out, visited = [], set()
+        stack = [t.grad_fn for t in reversed(list(res) + list(funcs) + list(aux))
+                 if isinstance(t, torch.Tensor) and t.grad_fn is not None]
+        while stack:
+            fn = stack.pop()
+            if fn is None or fn in visited:
+                continue
+            visited.add(fn)
+            leaf = getattr(fn, "variable", None)          # AccumulateGrad: a leaf that requires grad
+            if leaf is not None and id(leaf) not in seen:
+                seen.add(id(leaf))
+                out.append(leaf)
+            stack.extend(f for f, _ in reversed(fn.next_functions))
+        return out
 
     def parameters_linked(self):
         esz = self.theta.element_size()
@@ -122,8 +156,8 @@ class EagerProblem:
             raise ValueError("all coordinate vectors must have the same number of points")
         return cols
 
-    def _evaluate(self, coords, need_graph=True):
-        cols = self._columns(coords)
+    def _evaluate(self, coords, need_graph=True, cols=None):
+        cols = self._columns(coords) if cols is None else cols
         with torch.enable_grad():
             funcs = []
             for k, (net, cond) in enumerate(zip(self.nets, self.conditions)):

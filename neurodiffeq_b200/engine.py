@@ -48,7 +48,7 @@ class PjSpec(ctypes.Structure):
                 ("dir", (ctypes.c_float * PJ_MAX_COORDS) * PJ_MAX_DIRS),
                 ("n_funcs", ctypes.c_int32), ("n_eq", ctypes.c_int32), ("n_yrows", ctypes.c_int32),
                 ("n_slots", ctypes.c_int32), ("n_theta", ctypes.c_int64), ("net", PjNet * PJ_MAX_NETS),
-                ("n3", ctypes.c_int32), ("net_more", PjNet * (PJ_MAX_NETS_ALL - PJ_MAX_NETS)),
+                ("n3", ctypes.c_int32), ("n_coef", ctypes.c_int32), ("net_more", PjNet * (PJ_MAX_NETS_ALL - PJ_MAX_NETS)),
                 ("deep", PjNetDeep * PJ_MAX_NETS_ALL)]
 
     def net_at(self, n):
@@ -286,6 +286,8 @@ class FusedProblem:
 
     # ---- parameters: one flat buffer of the problem's dtype, nn.Parameters become views (torch layout preserved) -------
     def _adopt_parameters(self):
+        """theta = [network parameters | trainable coefficients]: the coefficients' tensors (``TracedProblem.coef_tensors``,
+        whole, element by element) after every network parameter, so that they are the last ``n_coef`` entries."""
         params, seen = [], set()
         for nd in self.tp.nets:   # a module evaluated at two coordinate lists (boundary instance) owns ONE set of weights
             nd.module.to(device=self.device, dtype=self.dtype)
@@ -293,6 +295,11 @@ class FusedProblem:
                 if id(p) not in seen:
                     seen.add(id(p))
                     params.append(p)
+        for t in self.tp.coef_tensors:
+            if id(t) in seen:
+                raise NotImplementedError("a network parameter used as a coefficient of the equations")
+            params.append(t)
+        self.n_coef = self.tp.n_coef
         n_theta = sum(p.numel() for p in params)
         self.theta = torch.empty(n_theta, dtype=self.dtype, device=self.device)
         # one buffer [grad_theta | sum r^2] so that a multi-GPU step needs a single all-reduce (SURVEY.md §8e)
@@ -355,6 +362,7 @@ class FusedProblem:
         sp.n_slots = max(self._program(p).n_slots for p in (tp.prog_eval, tp.prog_train, tp.prog_train_ext) +
                          ((tp.prog_w,) if tp.wl else ()))
         sp.n_theta = self.n_theta
+        sp.n_coef = self.n_coef
         for n, nd in enumerate(tp.nets):
             net = sp.net_at(n)
             net.n_in = nd.widths[0]
@@ -374,6 +382,8 @@ class FusedProblem:
         key, and per Resnet instance the index tensors its gradient needs (made once: nothing is uploaded per step)."""
         tp, dev = self.tp, self.device
         self._theta_index, self._patch_sets, self._skips = {}, [], []
+        for key, k in tp.coef_index.items():     # coefficient k is theta[n_theta - n_coef + k]
+            self._theta_index[key] = self.n_theta - self.n_coef + k
         for k, nd in enumerate(tp.nets):
             if nd.skip is None:
                 continue
@@ -613,7 +623,7 @@ class FusedProblem:
             if self.f64:
                 raise ValueError("the specialised kernel is float32 only (this problem runs in float64)")
             if self._patch_sets:
-                raise ValueError("the program has trainable immediates (Resnet shortcut)")
+                raise ValueError("the program has trainable immediates (Resnet shortcut, equation coefficients)")
             if any(len(nd.linears) > PJ_MAX_LINEAR for nd in self.tp.nets):
                 raise ValueError(f"a network has more than {PJ_MAX_LINEAR} Linear layers (the tensor-core kernels take at most "
                                  f"{PJ_MAX_LINEAR})")

@@ -222,7 +222,8 @@ class BaseSolver:
         self._device_loop_state = None
         if self.device_loop and optimizer is None and self.dtype == torch.float32:   # the reference default (Adam, lr 1e-3) on the flat buffers, capturable
             from .optim import FlatAdam
-            self.optimizer = FlatAdam(self.problem.theta, self.problem.grad, capturable=True)
+            n = self._n_net_theta()   # like that default, the networks' parameters only: not the equation coefficients
+            self.optimizer = FlatAdam(self.problem.theta[:n], self.problem.grad[:n], capturable=True)
 
     # ---- hooks for subclasses -----------------------------------------------------------------------------------------
     def _traced_diff_eqs(self, *variables):
@@ -312,6 +313,10 @@ class BaseSolver:
     @property
     def batch(self):
         return self._batch
+
+    def _n_net_theta(self):
+        """Entries of the flat parameter buffer that belong to the networks; the trainable equation coefficients follow."""
+        return self.problem.theta.numel() - getattr(self.problem, "n_coef", 0)
 
     @property
     def best_nets(self):
@@ -716,9 +721,10 @@ class BaseSolver:
         fp = self.problem
         aux = fp.tp.aux_rows              # 'h1 semi': the user's residuals are auxiliary rows of u, not loss rows
         flat = [c.reshape(-1) for c in coords]
-        if best and self.best_nets_theta is not None:
+        if best and self.best_nets_theta is not None:   # the best networks with the live coefficients, as the reference
             live = fp.theta.clone()
-            fp.theta.copy_(self.best_nets_theta)
+            n = self._n_net_theta()
+            fp.theta[:n].copy_(self.best_nets_theta[:n])
             u, r, _ = fp.forward(flat, want_u=bool(aux), want_residual=not aux)
             fp.theta.copy_(live)
             fp.pack()

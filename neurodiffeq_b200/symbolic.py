@@ -31,6 +31,7 @@ OP_ST_U, OP_ST_R, OP_ST_SEED = 20, 21, 22
 OP_TAN, OP_SINH, OP_COSH, OP_ATAN, OP_ERF = 23, 24, 25, 26, 27
 OP_ST_W = 28   # store a per-point weight of the combined second-order channel
 OP_POW = 29    # slot ** slot: double programs only (an exponent float32 cannot hold, Program.to_f64)
+OP_ST_COT = 30  # add a per-point cotangent dL/d(coefficient k) to the forward kernel's batch sum of coefficient k
 
 _UNARY = {"neg": OP_NEG, "sin": OP_SIN, "cos": OP_COS, "exp": OP_EXP, "log": OP_LOG, "tanh": OP_TANH,
           "sqrt": OP_SQRT, "abs": OP_ABS, "sign": OP_SIGN, "rcp": OP_RCP, "tan": OP_TAN, "sinh": OP_SINH,
@@ -54,6 +55,7 @@ class Graph:
         self._net_ids = {}
         self.n_sampled = None   # number of sampled coordinates (set by the tracer); constant coordinates follow them
         self.const_coords = []  # values of the constant ("virtual") coordinates n_sampled, n_sampled + 1, ...
+        self.coef_tensors = []  # trainable tensors whose elements are coefficients of the trace, in order of first use
 
     def _mk(self, op, args=(), imm=None):
         key = (op, tuple(a.idx for a in args), imm)
@@ -95,9 +97,32 @@ class Graph:
 
     def theta(self, key):
         """A trainable scalar that enters the residual program directly (not through a network jet): the entries of a
-        Resnet's bias-free shortcut matrix.  Constant w.r.t. the coordinates; lowered as an OP_CONST whose immediate the
-        engine re-writes whenever the parameters change (``Program.patch``)."""
+        Resnet's bias-free shortcut matrix, and the user's equation coefficients (:meth:`coefficient`).  Constant w.r.t. the
+        coordinates; lowered as an OP_CONST whose immediate the engine re-writes whenever the parameters change
+        (``Program.patch``)."""
         return self._mk("theta", (), key)
+
+    def coefficient(self, x):
+        """The ``theta`` leaf of a trainable coefficient: a one-element tensor that requires grad and is either a leaf
+        (``nn.Parameter(torch.tensor(0.5))``) or a one-element view of one (``c[0]`` of ``c = nn.Parameter(torch.zeros(3))``).
+        Key ``("coef", id(leaf), flat index)``; the leaf tensors are kept in ``coef_tensors``.  Anything else that requires
+        grad (a tensor computed from a trainable one, a multi-element view) raises ``NotImplementedError``."""
+        leaf = x if x.is_leaf else x._base
+        if x.numel() != 1 or leaf is None or not leaf.is_leaf or not leaf.requires_grad:
+            raise NotImplementedError(f"{describe_tensor(x)} requires grad but is not a trainable coefficient: the fused "
+                                      f"kernels train 1-element leaf tensors and 1-element views of leaf tensors only")
+        if leaf is x:
+            index = 0
+        else:
+            if x.dtype != leaf.dtype or not leaf.is_contiguous():
+                raise NotImplementedError(f"{describe_tensor(x)}: a coefficient must be an element of a contiguous tensor "
+                                          f"of the same dtype")
+            index = x.storage_offset() - leaf.storage_offset()
+            if not 0 <= index < leaf.numel():
+                raise NotImplementedError(f"{describe_tensor(x)}: not an element of its base tensor")
+        if not any(t is leaf for t in self.coef_tensors):
+            self.coef_tensors.append(leaf)
+        return self.theta(("coef", id(leaf), int(index)))
 
     def param(self, k):
         return self._mk("param", (), int(k))
@@ -118,6 +143,8 @@ class Graph:
             return self.const(x)
         if isinstance(x, np.ndarray) and x.size == 1:
             return self.const(float(x.reshape(-1)[0]))
+        if isinstance(x, torch.Tensor) and x.requires_grad:
+            return self.coefficient(x)
         if isinstance(x, torch.Tensor) and x.numel() == 1:
             return self.const(float(x.detach().reshape(-1)[0]))
         raise TypeError(f"cannot use {type(x).__name__} inside a traced (fused) expression; "
@@ -571,6 +598,12 @@ _DUNDER = {"__add__": ("add", False), "__radd__": ("add", True), "__sub__": ("su
            "__rtruediv__": ("div", True), "__div__": ("div", False), "__rdiv__": ("div", True), "__pow__": ("pow", False)}
 
 
+def describe_tensor(x):
+    """How a refusal names a tensor: shape, dtype and the operation that computed it."""
+    origin = "leaf" if x.grad_fn is None else type(x.grad_fn).__name__
+    return f"tensor(shape={tuple(x.shape)}, dtype={x.dtype}, {origin})"
+
+
 def _is_block(x):
     """An (N, k) operand: a traced block, or a tensor / array of k > 1 per-column constants."""
     return isinstance(x, SymColumns) or (isinstance(x, (torch.Tensor, np.ndarray)) and _numel(x) > 1)
@@ -588,6 +621,11 @@ def _column_values(x, width):
         if len(x.cols) == 1:
             return list(x.cols) * width
         raise ValueError(f"traced blocks of widths {len(x.cols)} and {width} do not broadcast")
+    if isinstance(x, torch.Tensor) and x.requires_grad:
+        if x.numel() == 1:
+            return [x] * width      # a trainable coefficient: Graph.lift makes it a theta leaf
+        raise NotImplementedError(f"{describe_tensor(x)} requires grad: a trainable tensor of several elements cannot "
+                                  f"enter a traced expression (use its elements, c[0], c[1], ..., as coefficients)")
     if isinstance(x, (torch.Tensor, np.ndarray)):
         a = x.detach().cpu().double().numpy() if isinstance(x, torch.Tensor) else np.asarray(x, dtype=np.float64)
         if a.size == 1:
@@ -1176,13 +1214,15 @@ def depends_on_jets(expr):
     return any(n.op in ("net", "ych") for n in topo_order([expr]))
 
 
-def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n_seed=0, n_w=0, theta=None):
+def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n_seed=0, n_w=0, theta=None, n_cot=0):
     """Pure-numpy interpreter of the bytecode (host-side check of the lowering; float64).  ``theta``: values of the
     trainable scalars the program's patched constants stand for (``Program.patch`` keys -> float).  Float programs take
-    their immediates from ``exact_imm``; double programs (``Program.to_f64``) are decoded from the code alone."""
+    their immediates from ``exact_imm``; double programs (``Program.to_f64``) are decoded from the code alone.
+    ``n_cot > 0``: also return the per-point coefficient cotangents [n_cot, N] (OP_ST_COT) as a fourth result."""
     n = coords.shape[1]
     val = np.zeros((program.n_slots, n))
     u, r, seed = np.zeros((n_u, n)), np.zeros((n_r, n)), np.zeros((n_seed, n))
+    cot = np.zeros((n_cot, n))
     wout = np.zeros((n_w, n))
     bits = lambda b: float(np.array([b], dtype=np.int32).view(np.float32)[0])  # noqa: E731
     un = {OP_NEG: np.negative, OP_SIN: np.sin, OP_COS: np.cos, OP_EXP: np.exp, OP_LOG: np.log, OP_TANH: np.tanh,
@@ -1225,8 +1265,10 @@ def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n
             seed[dst] = val[a]
         elif op == OP_ST_W:
             wout[dst] = val[a]
+        elif op == OP_ST_COT:
+            cot[dst] += val[a]
         else:
             val[dst] = un[op](val[a])
     if n_w:
         return wout
-    return u, r, seed
+    return (u, r, seed, cot) if n_cot else (u, r, seed)

@@ -205,6 +205,15 @@ class TracedProblem:
 
         yrow = lambda net_idx, o, c: self.yrow0[net_idx] + o * C + c  # noqa: E731
         self._yrow = yrow
+        # trainable coefficients (Graph.coefficient): their tensors follow the network parameters in the flat theta, element
+        # by element; coef_index[key] is the position of a coefficient in that tail
+        self.coef_tensors = list(g.coef_tensors)
+        self.coef_index, off = {}, 0
+        for t in self.coef_tensors:
+            for i in range(t.numel()):
+                self.coef_index[("coef", id(t), i)] = off + i
+            off += t.numel()
+        self.n_coef = off
         self.prog_w = S.lower([(S.OP_ST_W, row, e) for row, e in self.weight_exprs], yrow) if self.wl else None
         # --- programs ---------------------------------------------------------------------------------------------------
         self.prog_eval = S.lower([(S.OP_ST_U, k, f) for k, f in enumerate(self.funcs)]
@@ -245,8 +254,9 @@ class TracedProblem:
             for leaf, coef in S.reverse_gradients([(r, g.const(1.0))]).items():
                 if not is_sec(leaf):
                     continue
-                if S.depends_on_jets(coef):
-                    return                       # not affine in the second derivatives / jet-dependent coefficient
+                if S.depends_on_jets(coef) or any(n.op == "theta" and n.imm[0] == "coef" for n in S.topo_order([coef])):
+                    return                       # not affine in the second derivatives / jet-dependent coefficient / a
+                    #                              trainable coefficient (the train program could not see its cotangent)
                 net_idx, o, c = leaf.imm
                 if owner.setdefault(net_idx, (e, o)) != (e, o):
                     return                       # two equations / outputs need different combinations of one net's jets
@@ -274,12 +284,16 @@ class TracedProblem:
                 cots += [(f, g.rbar(self.n_eq + k)) for k, f in enumerate(self.funcs)]
         else:  # L = scale/2 * sum r^2 with scale = 2/(N n_eq)  ->  dL/dr = scale * r
             cots = [(r, g.mul(g.param(S.PARAM_LOSS_SCALE), r)) for r in self.residuals]
-        adj = S.reverse_gradients(cots)
-        by_row = {self._yrow(*leaf.imm): expr for leaf, expr in adj.items()}
+        is_coef = lambda n: n.op == "theta" and n.imm[0] == "coef"  # noqa: E731
+        adj = S.reverse_gradients(cots, wrt_filter=lambda n: n.op in ("net", "ych") or is_coef(n))
+        by_row = {self._yrow(*leaf.imm): expr for leaf, expr in adj.items() if not is_coef(leaf)}
         outs = [(S.OP_ST_R, e, r) for e, r in enumerate(self.residuals)]
         zero = g.const(0.0)
         for row in range(self.n_yrows):
             outs.append((S.OP_ST_SEED, row, by_row.get(row, zero)))
+        # per-point cotangents of the coefficients; the forward kernel sums them over the batch
+        outs += sorted(((S.OP_ST_COT, self.coef_index[leaf.imm], expr) for leaf, expr in adj.items() if is_coef(leaf)),
+                       key=lambda o: o[1])
         return S.lower(outs, self._yrow)
 
     @property

@@ -20,7 +20,8 @@ import torch
 Workload = namedtuple(
     "Workload",
     "name solver coord_names coord_ranges nets_spec make_nets make_conditions diff_eqs n_eq default_n flops_fwdjet "
-    "eq_param_index"
+    "eq_param_index make_coefficients",
+    defaults=(None,)
 )
 
 NU_BURGERS = 0.01 / math.pi
@@ -582,6 +583,107 @@ def _d4(nd):
                     K, 16384, sum(_fcnn_flops(w, 2) for w, _ in shapes), None)
 
 
+# ----------------------------------------------------------------------------------------------------------------------
+# I1..I4  inverse (parameter-identification) problems: unknown equation coefficients are trainable tensors, used in
+# diff_eqs (and in a condition's boundary value), trained with the networks.  make_coefficients() makes fresh tensors
+# that the equations and conditions of the workload share; call it before tracing or evaluating them.
+# ----------------------------------------------------------------------------------------------------------------------
+def _coefficient_box(*values):
+    box = []
+
+    def make_coefficients():
+        box[:] = [torch.nn.Parameter(torch.tensor(v, dtype=torch.get_default_dtype())) for v in values]
+        return list(box)
+
+    return box, make_coefficients
+
+
+def _i1(nd):
+    """Raissi's Burgers identification: u_t + l1 u u_x - l2 u_xx = 0 with l1, l2 unknown (IBVP1D, zero ends)."""
+    lam, make_coefficients = _coefficient_box(0.5, 0.02)
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(32, 32))]
+
+    def make_conditions():
+        return [nd.IBVP1D(x_min=-1, x_max=1, t_min=0, t_min_val=lambda x: -torch.sin(np.pi * x),
+                          x_min_val=lambda t: 0, x_max_val=lambda t: 0)]
+
+    def diff_eqs(u, x, t):
+        return [nd.diff(u, t) + lam[0] * u * nd.diff(u, x) - lam[1] * nd.diff(u, x, order=2)]
+
+    shape = (2, 32, 32, 1)
+    return Workload("i1_burgers_identification", "Solver2D", ("x", "t"), ((-1.0, 1.0), (0.0, 1.0)), [(shape, "tanh")],
+                    make_nets, make_conditions, diff_eqs, 1, 16384, _fcnn_flops(shape, 4), None, make_coefficients)
+
+
+def _i2(nd):
+    """Lotka-Volterra with unknown alpha, beta, gamma, delta: u' = alpha u - beta u v, v' = delta u v - gamma v."""
+    c, make_coefficients = _coefficient_box(1.2, 0.8, 0.9, 1.1)
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(32, 32)) for _ in range(2)]
+
+    def make_conditions():
+        return [nd.IVP(t_0=0.0, u_0=1.5), nd.IVP(t_0=0.0, u_0=1.0)]
+
+    def diff_eqs(u, v, t):
+        alpha, beta, gamma, delta = c
+        return [nd.diff(u, t) - (alpha * u - beta * u * v), nd.diff(v, t) - (delta * u * v - gamma * v)]
+
+    shape = (1, 32, 32, 1)
+    return Workload("i2_lotka_volterra_identification", "Solver1D", ("t",), ((0.1, 6.0),), [(shape, "tanh")] * 2,
+                    make_nets, make_conditions, diff_eqs, 2, 1024, 2 * _fcnn_flops(shape, 2), None, make_coefficients)
+
+
+def _i3(nd):
+    """Heat equation with an unknown decay rate k, u_t - 0.3 u_xx + k u = 0, and an unknown amplitude a of the initial
+    value a sin(pi x / 2) (a coefficient inside a condition), Dirichlet at x = 0 and Neumann at x = 1 (a boundary network
+    instance).  Both terms with derivatives in t or x carry second-order jets of the boundary instance, and the four jet
+    directions of this problem need the combined second-order channel, whose weights must not depend on a coefficient:
+    so the unknown rate multiplies u, not u_t or u_xx."""
+    c, make_coefficients = _coefficient_box(0.5, 0.9)
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(32, 32))]
+
+    def make_conditions():
+        return [nd.IBVP1D(x_min=0.0, x_max=1.0, t_min=0.0, t_min_val=lambda x: c[1] * torch.sin(0.5 * np.pi * x),
+                          x_min_val=lambda t: 0.2 * torch.sin(t), x_max_prime=lambda t: 0.1 * t)]
+
+    def diff_eqs(u, x, t):
+        return [nd.diff(u, t) - 0.3 * nd.diff(u, x, order=2) + c[0] * u]
+
+    shape = (2, 32, 32, 1)
+    return Workload("i3_heat_identification_neumann", "Solver2D", ("x", "t"), ((0.0, 1.0), (0.0, 1.0)),
+                    [(shape, "tanh")], make_nets, make_conditions, diff_eqs, 1, 16384, 2 * _fcnn_flops(shape, 9), None,
+                    make_coefficients)
+
+
+def _i4(nd):
+    """Damped oscillator u'' + c[0] u' + c[1] u = 0, u(0) = 1, u'(0) = 0, with the coefficients elements of ONE vector
+    parameter c."""
+    box = []
+
+    def make_coefficients():
+        box[:] = [torch.nn.Parameter(torch.tensor([0.3, 2.0], dtype=torch.get_default_dtype()))]
+        return list(box)
+
+    def make_nets():
+        return [nd.FCNN(n_input_units=1, n_output_units=1, hidden_units=(32, 32))]
+
+    def make_conditions():
+        return [nd.IVP(t_0=0.0, u_0=1.0, u_0_prime=0.0)]
+
+    def diff_eqs(u, t):
+        c = box[0]
+        return [nd.diff(u, t, order=2) + c[0] * nd.diff(u, t) + c[1] * u]
+
+    shape = (1, 32, 32, 1)
+    return Workload("i4_oscillator_vector_coefficients", "Solver1D", ("t",), ((0.0, 3.0),), [(shape, "tanh")],
+                    make_nets, make_conditions, diff_eqs, 1, 1024, _fcnn_flops(shape, 3), None, make_coefficients)
+
+
 _EXTRA = {
     "x1": lambda nd: _heat(nd, "x1_heat_dirichlet_neumann", "right"),
     "x2": lambda nd: _heat(nd, "x2_heat_neumann_dirichlet", "left"),
@@ -626,6 +728,10 @@ _BUILDERS.update(_ACTIVATION)
 _DEEP = {"d1": _d1, "d2": _d2, "d3": _d3, "d4": _d4}
 DEEP_NAMES = tuple(_DEEP)
 _BUILDERS.update(_DEEP)
+# inverse problems: trainable equation coefficients (Workload.make_coefficients); kept out of the tuples above as well
+_INVERSE = {"i1": _i1, "i2": _i2, "i3": _i3, "i4": _i4}
+INVERSE_NAMES = tuple(_INVERSE)
+_BUILDERS.update(_INVERSE)
 # workloads whose conditions see only the first coordinate (a network of r alone, as SolverSpherical passes it)
 _RADIAL = ("s1", "s2")
 
@@ -727,6 +833,8 @@ def build_fused(key, params=None, seed=0, device=None):
     from neurodiffeq_b200.engine import FusedProblem
     wl = build(product_namespace(), key)
     torch.manual_seed(seed)
+    if wl.make_coefficients is not None:
+        wl.make_coefficients()
     nets, conds = wl.make_nets(), wl.make_conditions()
     if params is not None:
         set_params(nets, params)
