@@ -189,6 +189,50 @@ int pj_forward_train_jit(void* cu_function, const PjSpec* spec, const int32_t* p
                          const float* theta_pack, float loss_scale, float* resid_out, float* sumsq_out, void* workspace,
                          size_t workspace_bytes, void* stream);
 
+/* ---- coordinate-only field rows (irregular domains: pde.CustomBoundaryCondition, reference pde.py:442-789) -------------
+ * Programs of such problems read per-point values of thin-plate-spline (TPS) maps and their derivatives with OP_FIELD row:
+ * fields[row * n_points + i].  pj_tps_fields fills those rows; the _fields variants of the forward entry points pass them
+ * to the program (the plain entry points pass NULL, and their programs must not contain OP_FIELD).
+ * A group is a set of M centres (x_i, y_i) with K maps over them, map k = coefs[k][0 .. M + 2] = [c_1..c_M, c_0, c_x, c_y]:
+ *     T_k(x, y) = sum_i c_i q_i ln q_i + c_0 + c_x x + c_y y,   q_i = (x - x_i)^2 + (y - y_i)^2 + s2,  s2 > 0,
+ * with x = coordinate coord_x and y = coordinate coord_y.  Row r of the output is derivative rows[r].deriv of map
+ * rows[r].map of group rows[r].group: 0 value, 1 d/dx, 2 d/dy, 3 d2/dx2, 4 d2/dxdy, 5 d2/dy2.  Centres and coefficients are
+ * device arrays of the call's element type; out is [n_rows][n_points].  No allocation, one launch on `stream`,
+ * CUDA-graph capturable; the result is run-to-run identical (centres summed in order, no atomics). */
+#define PJ_MAX_TPS_GROUPS 8
+#define PJ_MAX_FIELD_ROWS 64
+typedef struct PjTpsGroup {
+    const void* centres;                /* device, [n_centres][2]                                                             */
+    const void* coefs;                  /* device, [n_maps][n_centres + 3]                                                    */
+    int32_t n_centres, n_maps;
+    int32_t coord_x, coord_y;           /* coordinates the maps are functions of                                              */
+    double s2;                          /* squared stiffness                                                                  */
+} PjTpsGroup;
+typedef struct PjFieldRow {
+    int32_t group, map, deriv, pad_;
+} PjFieldRow;
+int pj_tps_fields(const PjTpsGroup* groups /*host*/, int32_t n_groups, const PjFieldRow* rows /*host*/, int32_t n_rows,
+                  const float* const* coords /*host array of device ptrs*/, int32_t n_coords, int64_t n_points,
+                  float* out /*device*/, void* stream);
+int pj_tps_fields_f64(const PjTpsGroup* groups, int32_t n_groups, const PjFieldRow* rows, int32_t n_rows,
+                      const double* const* coords, int32_t n_coords, int64_t n_points, double* out, void* stream);
+int pj_forward_fields(const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w,
+                      int32_t prog_w_len, const float* const* coords, int64_t n_points, const float* theta_pack,
+                      const float* fields /*device, pj_tps_fields*/, float* u_out, float* resid_out, float* sumsq_out,
+                      void* workspace, size_t workspace_bytes, void* stream);
+int pj_forward_train_fields(const PjSpec* spec, const int32_t* prog_train, int32_t prog_len, const int32_t* prog_w,
+                            int32_t prog_w_len, const float* const* coords, int64_t n_points, const float* theta_pack,
+                            const float* fields, float loss_scale, const float* rbar, float* resid_out, float* sumsq_out,
+                            void* workspace, size_t workspace_bytes, void* stream);
+int pj_forward_fields_f64(const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w,
+                          int32_t prog_w_len, const double* const* coords, int64_t n_points, const double* theta_pack,
+                          const double* fields, double* u_out, double* resid_out, double* sumsq_out, void* workspace,
+                          size_t workspace_bytes, void* stream);
+int pj_forward_train_fields_f64(const PjSpec* spec, const int32_t* prog_train, int32_t prog_len, const int32_t* prog_w,
+                                int32_t prog_w_len, const double* const* coords, int64_t n_points, const double* theta_pack,
+                                const double* fields, double loss_scale, const double* rbar, double* resid_out,
+                                double* sumsq_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Reverse pass: grad_theta += dL/dtheta  (replaces loss.backward(), solvers.py:393).
  * Must follow pj_forward_train on the same workspace / points / theta_pack.                                    */
 int pj_backward(const PjSpec* spec, const float* const* coords, int64_t n_points, const float* theta_pack,

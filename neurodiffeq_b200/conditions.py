@@ -19,6 +19,7 @@ The Neumann flavours evaluate the network AT a boundary abscissa
 """
 import warnings
 
+import numpy as np
 import torch
 
 from . import symbolic as _sym
@@ -87,6 +88,14 @@ class BaseCondition:
         warnings.warn(f"`{self.__class__.__name__}.set_impose_on` is deprecated and will be removed in the future",
                       DeprecationWarning)
         self.ith_unit = ith_unit
+
+
+class IrregularBoundaryCondition(BaseCondition):
+    """Base class of conditions on irregular domains (reference conditions.py:138-154); see ``pde.CustomBoundaryCondition``."""
+
+    def in_domain(self, *coordinates):
+        """Whether each point lies inside the domain, as a bool array of the first coordinate's shape: every point, here."""
+        return np.ones_like(np.asarray(coordinates[0]), dtype=bool)
 
 
 class NoCondition(BaseCondition):

@@ -48,6 +48,7 @@ def build(force=False, verbose=False, extra_flags=(), lib=None, objdir_name="bui
             (os.path.join(objdir, "comm.o"), os.path.join(HERE, "pinnjet_comm.cu"), list(extra_flags)),
             (os.path.join(objdir, "sample.o"), os.path.join(HERE, "pinnjet_sample.cu"), list(extra_flags)),
             (os.path.join(objdir, "optim.o"), os.path.join(HERE, "pinnjet_optim.cu"), list(extra_flags)),
+            (os.path.join(objdir, "tps.o"), os.path.join(HERE, "pinnjet_tps.cu"), list(extra_flags)),
             (os.path.join(objdir, "inst_common.o"), os.path.join(HERE, "pinnjet_inst.cu"),
              ["-DPJ_N1=-1", "-DPJ_N2=-1"] + list(extra_flags))]
     # float kernels, then the double FFMA kernels of the same scheme (same source, PJ_F64=1); each once more with the

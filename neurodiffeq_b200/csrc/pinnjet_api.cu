@@ -11,6 +11,7 @@
 #include <cuda_bf16.h>
 
 #include "pinnjet_tc.cuh"
+#include "pinnjet_tps.cuh"
 
 namespace pj {
 
@@ -385,7 +386,8 @@ template <typename R>
 static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, const int32_t* prog_w, int32_t prog_w_len,
                   const R* const* coords, int64_t n,
                   const R* theta_pack, int mode, R loss_scale, const R* rbar, R* u_out, R* r_out,
-                  R* sumsq_out, void* ws, size_t ws_bytes, void* stream, void* jit_function = nullptr) {
+                  R* sumsq_out, void* ws, size_t ws_bytes, void* stream, void* jit_function = nullptr,
+                  const R* fields = nullptr) {
     if (!spec || !prog || !coords || !theta_pack || !ws) return fail(-1, "null argument");
     typename ArgsOf<R>::K1 a;
     memset(&a, 0, sizeof(a));
@@ -412,6 +414,7 @@ static int run_k1(const PjSpec* spec, const int32_t* prog, int32_t prog_len, con
     a.rbar = rbar;
     a.u_out = u_out;
     a.r_out = r_out;
+    a.fields = fields;
     char* w = static_cast<char*>(ws);
     a.loss_part = reinterpret_cast<R*>(w + a.plan.ws_loss);
     a.dbg = reinterpret_cast<float*>(w + a.plan.ws_loss) + LOSS_DBG_WORD;
@@ -480,6 +483,39 @@ int pj_forward_train_f64(const PjSpec* spec, const int32_t* prog_train, int32_t 
                          size_t workspace_bytes, void* stream) {
     return run_k1<double>(spec, prog_train, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 1, loss_scale, rbar, nullptr,
                           resid_out, sumsq_out, workspace, workspace_bytes, stream);
+}
+
+int pj_forward_fields(const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w,
+                      int32_t prog_w_len, const float* const* coords, int64_t n_points, const float* theta_pack,
+                      const float* fields, float* u_out, float* resid_out, float* sumsq_out, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+    if (!fields) return fail(-1, "null field rows");
+    return run_k1<float>(spec, prog_eval, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 0, 0.0f, nullptr, u_out, resid_out,
+                         sumsq_out, workspace, workspace_bytes, stream, nullptr, fields);
+}
+int pj_forward_fields_f64(const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w,
+                          int32_t prog_w_len, const double* const* coords, int64_t n_points, const double* theta_pack,
+                          const double* fields, double* u_out, double* resid_out, double* sumsq_out, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+    if (!fields) return fail(-1, "null field rows");
+    return run_k1<double>(spec, prog_eval, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 0, 0.0, nullptr, u_out, resid_out,
+                          sumsq_out, workspace, workspace_bytes, stream, nullptr, fields);
+}
+int pj_forward_train_fields(const PjSpec* spec, const int32_t* prog_train, int32_t prog_len, const int32_t* prog_w,
+                            int32_t prog_w_len, const float* const* coords, int64_t n_points, const float* theta_pack,
+                            const float* fields, float loss_scale, const float* rbar, float* resid_out, float* sumsq_out,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+    if (!fields) return fail(-1, "null field rows");
+    return run_k1<float>(spec, prog_train, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 1, loss_scale, rbar, nullptr,
+                         resid_out, sumsq_out, workspace, workspace_bytes, stream, nullptr, fields);
+}
+int pj_forward_train_fields_f64(const PjSpec* spec, const int32_t* prog_train, int32_t prog_len, const int32_t* prog_w,
+                                int32_t prog_w_len, const double* const* coords, int64_t n_points, const double* theta_pack,
+                                const double* fields, double loss_scale, const double* rbar, double* resid_out,
+                                double* sumsq_out, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!fields) return fail(-1, "null field rows");
+    return run_k1<double>(spec, prog_train, prog_len, prog_w, prog_w_len, coords, n_points, theta_pack, 1, loss_scale, rbar, nullptr,
+                          resid_out, sumsq_out, workspace, workspace_bytes, stream, nullptr, fields);
 }
 
 int pj_forward_jit(void* cu_function, const PjSpec* spec, const int32_t* prog_eval, int32_t prog_len, const int32_t* prog_w,
@@ -573,6 +609,56 @@ int pj_backward_allreduce(const PjSpec* spec, const float* const* coords, int64_
     return check_cuda(launch_reduce_allreduce(reinterpret_cast<const unsigned long long*>(peer_buffers), rank, world, gpart, n_parts,
                                               spec->n_theta, gradbuf, spec->n_theta + n_tail, (cudaStream_t)stream),
                       "reduce + all-reduce launch");
+}
+
+}  // extern "C"
+
+// ---- field kernel (pinnjet_tps.cu): the caller's descriptors, checked, as the kernel's argument ----------------------
+template <typename R>
+static int tps_fields_impl(const PjTpsGroup* groups, int32_t n_groups, const PjFieldRow* rows, int32_t n_rows,
+                           const R* const* coords, int32_t n_coords, int64_t n_points, R* out, void* stream) {
+    if (!groups || !rows || !coords || !out) return fail(-1, "null argument");
+    if (n_groups < 1 || n_groups > PJ_MAX_TPS_GROUPS) return fail(-1, "%d TPS groups (1 to %d)", n_groups, PJ_MAX_TPS_GROUPS);
+    if (n_rows < 1 || n_rows > PJ_MAX_FIELD_ROWS) return fail(-1, "%d field rows (1 to %d)", n_rows, PJ_MAX_FIELD_ROWS);
+    if (n_coords < 1 || n_coords > PJ_MAX_COORDS) return fail(-1, "%d coordinates (1 to %d)", n_coords, PJ_MAX_COORDS);
+    if (n_points < 1) return fail(-1, "n_points = %lld", (long long)n_points);
+    TpsArgs<R> a;
+    memset(&a, 0, sizeof(a));
+    for (int i = 0; i < n_coords; ++i) {
+        if (!coords[i]) return fail(-1, "coords[%d] is null", i);
+        a.coords[i] = coords[i];
+    }
+    for (int g = 0; g < n_groups; ++g) {
+        const PjTpsGroup& G = groups[g];
+        if (!G.centres || !G.coefs || G.n_centres < 1 || G.n_maps < 1 || !(G.s2 > 0.0) || G.coord_x < 0 || G.coord_x >= n_coords ||
+            G.coord_y < 0 || G.coord_y >= n_coords)
+            return fail(-1, "TPS group %d: null arrays, no centres or maps, s2 <= 0 or a coordinate out of range", g);
+        a.group[g] = TpsGroupK<R>{static_cast<const R*>(G.centres), static_cast<const R*>(G.coefs), G.n_centres, G.n_maps,
+                                  G.coord_x, G.coord_y, R(G.s2)};
+    }
+    for (int r = 0; r < n_rows; ++r) {
+        const PjFieldRow& row = rows[r];
+        if (row.group < 0 || row.group >= n_groups || row.map < 0 || row.map >= groups[row.group].n_maps || row.deriv < 0 ||
+            row.deriv > 5)
+            return fail(-1, "field row %d: group %d, map %d, derivative %d out of range", r, row.group, row.map, row.deriv);
+        a.row[r] = make_int4(row.group, row.map, row.deriv, 0);
+    }
+    a.n = n_points;
+    a.n_groups = n_groups;
+    a.n_rows = n_rows;
+    a.out = out;
+    return check_cuda(launch_tps_fields(a, (cudaStream_t)stream), "field kernel launch");
+}
+
+extern "C" {
+
+int pj_tps_fields(const PjTpsGroup* groups, int32_t n_groups, const PjFieldRow* rows, int32_t n_rows, const float* const* coords,
+                  int32_t n_coords, int64_t n_points, float* out, void* stream) {
+    return tps_fields_impl(groups, n_groups, rows, n_rows, coords, n_coords, n_points, out, stream);
+}
+int pj_tps_fields_f64(const PjTpsGroup* groups, int32_t n_groups, const PjFieldRow* rows, int32_t n_rows,
+                      const double* const* coords, int32_t n_coords, int64_t n_points, double* out, void* stream) {
+    return tps_fields_impl(groups, n_groups, rows, n_rows, coords, n_coords, n_points, out, stream);
 }
 
 }  // extern "C"

@@ -53,7 +53,8 @@ enum : int {
     OP_CONST = 0, OP_COORD, OP_NET, OP_RBAR, OP_PARAM, OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_NEG, OP_SIN, OP_COS, OP_EXP,
     OP_LOG, OP_TANH, OP_SQRT, OP_ABS, OP_SIGN, OP_POWC, OP_RCP, OP_ST_U, OP_ST_R, OP_ST_SEED, OP_TAN, OP_SINH, OP_COSH,
     OP_ATAN, OP_ERF, OP_ST_W, OP_POW,  // OP_POW: double programs only
-    OP_ST_COT                          // per-point cotangent of a trainable coefficient (train programs)
+    OP_ST_COT,                         // per-point cotangent of a trainable coefficient (train programs)
+    OP_FIELD                           // row of the coordinate-only field table at the point (pj_tps_fields)
 };
 
 // Network instance n as the FFMA kernels index it: PJ_SPEC_NET(&spec, n) with the layers of spec.deep[n] in the same
@@ -97,6 +98,7 @@ struct K1ArgsT {
     unsigned* ticket;                    // ... found by this counter (zero between launches; lives in the loss-partial block)
     R* coef_part;                        // train mode, spec.n_coef > 0: per-CTA cotangent sums [n_coef][max_loss_parts]
     R* coef_sum;                         // ... and their totals [n_coef], written by the same last warp (read by K2)
+    const R* fields;                     // field rows [n_rows][N] that OP_FIELD reads, or nullptr (no OP_FIELD)
 };
 
 template <typename R>

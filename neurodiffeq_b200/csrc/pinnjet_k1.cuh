@@ -194,6 +194,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
                     ProgIOT<R> io{A.coords, gidx, A.N, yb + bp, EB, A.rbar, A.loss_scale, A.u_out, A.r_out, seed_tile, T2};
                     io.cot = cot;
                     io.n_cot = n_coef;
+                    io.fields = A.fields;
                     my_sumsq += run_program<32>(prog_s, A.prog_len, slots + lane, io);
                 } else if (seed_tile) {
                     for (int r = 0; r < sp.n_yrows; ++r) seed_tile[r * T2] = 0.0f;   // padded points: zero adjoint
@@ -246,6 +247,7 @@ __device__ __forceinline__ void k1_forward_body(const K1ArgsT<R>& A) {
                 ProgIOT<R> io{A.coords, min(base + tid, A.N - 1), A.N, nullptr, 0, nullptr, 0.0f, nullptr, nullptr, nullptr, T2};
                 io.w_out = wbuf + tid;
                 io.w_stride = T;
+                io.fields = A.fields;
                 run_program<NTC>(progw_s, A.prog_w_len, wslots + tid, io);
             }
             bar_compute<NTC>();

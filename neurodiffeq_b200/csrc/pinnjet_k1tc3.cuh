@@ -149,7 +149,7 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
                         pj_jit_program_w(io);
                     } else {
                         run_program_rt(progw_s, A.prog_w_len, wslots + lane, A.coords, min(base + pt, A.N - 1), A.N, nullptr, 0,
-                                       nullptr, 0.0f, nullptr, nullptr, nullptr, TP, wb + pt, TP);
+                                       nullptr, 0.0f, nullptr, nullptr, nullptr, TP, wb + pt, TP, A.fields);
                     }
                 }
                 __syncwarp();
@@ -199,7 +199,7 @@ __device__ __forceinline__ void k1tc3_body(const K1Args& A) {
                         my_sumsq += train ? pj_jit_program_train(io) : pj_jit_program_eval(io);
                     } else {
                         my_sumsq += run_program_rt(prog_s, A.prog_len, my_slots, A.coords, gidx, A.N, yb + bp, K1T_EB, A.rbar,
-                                                   A.loss_scale, A.u_out, A.r_out, seed_tile, sT, nullptr, 0);
+                                                   A.loss_scale, A.u_out, A.r_out, seed_tile, sT, nullptr, 0, A.fields);
                     }
                 } else if (seed_tile) {
                     for (int r = 0; r < sp.n_yrows; ++r) seed_tile[r * sT] = 0.0f;   // padded points: zero adjoint

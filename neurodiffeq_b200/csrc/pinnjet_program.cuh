@@ -28,6 +28,7 @@ struct ProgIOT {
     int w_stride = 0;
     R* cot = nullptr;             // train programs with coefficients: OP_ST_COT k adds to cot[k * 32] (this lane's sums),
     int n_cot = 0;                // ... for 0 <= k < n_cot (spec.n_coef); other indices are ignored
+    const R* fields = nullptr;    // OP_FIELD row: fields[row * N + gidx] (pj_tps_fields)
 };
 using ProgIO = ProgIOT<float>;
 
@@ -57,6 +58,8 @@ __device__ __forceinline__ R run_program(const int4* __restrict__ prog, int len,
                 case OP_RBAR: v = __ldg(io.rbar + (long long)ins.z * io.N + io.gidx); break;
                 default: v = io.loss_scale; break;
             }
+        } else if (op == OP_FIELD) {
+            v = __ldg(io.fields + (long long)ins.z * io.N + io.gidx);
         } else if (op == OP_ST_W) {
             io.w_out[ins.y * io.w_stride] = slot[ins.z * SLOT_STRIDE];
             continue;
@@ -109,10 +112,11 @@ static __device__ __noinline__ float run_program_rt(const int4* prog, int len, f
                                                     const float* const* coords, long long gidx, long long N,
                                                     const float* ycache, int ystride, const float* rbar, float loss_scale,
                                                     float* u_out, float* r_out, float* seed_tile, int T, float* w_out,
-                                                    int w_stride) {
+                                                    int w_stride, const float* fields) {
     ProgIO io{coords, gidx, N, ycache, ystride, rbar, loss_scale, u_out, r_out, seed_tile, T};
     io.w_out = w_out;
     io.w_stride = w_stride;
+    io.fields = fields;
     return run_program<32>(prog, len, slot, io);
 }
 

@@ -122,6 +122,17 @@ def load_library():
     lib.pj_forward_f64.argtypes = lib.pj_forward.argtypes
     lib.pj_forward_train_f64.argtypes = [ctypes.c_double if t is f32 else t for t in lib.pj_forward_train.argtypes]
     lib.pj_backward_f64.argtypes = lib.pj_backward.argtypes
+    # coordinate-only field rows (irregular domains): the field kernel and the forward entry points that read its rows
+    lib.pj_tps_fields.argtypes = [ctypes.POINTER(PjTpsGroup), i32, ctypes.POINTER(PjFieldRow), i32, ctypes.POINTER(vp), i32,
+                                  i64, vp, vp]
+    lib.pj_tps_fields_f64.argtypes = lib.pj_tps_fields.argtypes
+    lib.pj_forward_fields.argtypes = lib.pj_forward.argtypes[:8] + [vp] + lib.pj_forward.argtypes[8:]
+    lib.pj_forward_fields_f64.argtypes = lib.pj_forward_fields.argtypes
+    lib.pj_forward_train_fields.argtypes = lib.pj_forward_train.argtypes[:8] + [vp] + lib.pj_forward_train.argtypes[8:]
+    lib.pj_forward_train_fields_f64.argtypes = [ctypes.c_double if t is f32 else t for t in lib.pj_forward_train_fields.argtypes]
+    for fn in (lib.pj_tps_fields, lib.pj_tps_fields_f64, lib.pj_forward_fields, lib.pj_forward_fields_f64,
+               lib.pj_forward_train_fields, lib.pj_forward_train_fields_f64):
+        fn.restype = ctypes.c_int
     for fn in (lib.pj_sizes, lib.pj_pack, lib.pj_forward, lib.pj_forward_train, lib.pj_backward, lib.pj_forward_jit,
                lib.pj_forward_train_jit, lib.pj_backward_allreduce, lib.pj_sizes_f64, lib.pj_plan_info_f64, lib.pj_pack_f64,
                lib.pj_pack_zero_f64, lib.pj_forward_f64, lib.pj_forward_train_f64, lib.pj_backward_f64):
@@ -134,7 +145,8 @@ def load_library():
 
 EXPORTED_SYMBOLS = ("pj_abi_version", "pj_last_error", "pj_sizes", "pj_plan_info", "pj_pack", "pj_forward", "pj_forward_train",
                     "pj_backward", "pj_allreduce_bytes", "pj_allreduce_oneshot", "pj_sample", "pj_adam_step", "pj_forward_jit",
-                    "pj_forward_train_jit", "pj_backward_allreduce_bytes", "pj_backward_allreduce", "pj_pack_zero")
+                    "pj_forward_train_jit", "pj_backward_allreduce_bytes", "pj_backward_allreduce", "pj_pack_zero",
+                    "pj_tps_fields", "pj_forward_fields", "pj_forward_train_fields")
 F64_SYMBOLS = ("pj_sizes_f64", "pj_plan_info_f64", "pj_pack_f64", "pj_pack_zero_f64", "pj_forward_f64", "pj_forward_train_f64",
                "pj_backward_f64")
 
@@ -174,6 +186,25 @@ def pad_scheme(n1, n2, n3=0):
         raise NotImplementedError(f"no compiled kernel for jet channels (n1={n1}, n2={n2}); "
                                   f"available: {SUPPORTED_SCHEMES}")
     return best
+
+
+class PjTpsGroup(ctypes.Structure):
+    _fields_ = [("centres", ctypes.c_void_p), ("coefs", ctypes.c_void_p), ("n_centres", ctypes.c_int32),
+                ("n_maps", ctypes.c_int32), ("coord_x", ctypes.c_int32), ("coord_y", ctypes.c_int32), ("s2", ctypes.c_double)]
+
+
+class PjFieldRow(ctypes.Structure):
+    _fields_ = [("group", ctypes.c_int32), ("map", ctypes.c_int32), ("deriv", ctypes.c_int32), ("pad_", ctypes.c_int32)]
+
+
+PJ_MAX_TPS_GROUPS = 8
+
+
+def field_derivative_code(alpha, coords):
+    """PjFieldRow.deriv of multi-index ``alpha`` of a TPS map over coordinates ``coords`` = (i, j): 0 value, 1 d/di,
+    2 d/dj, 3 d2/di2, 4 d2/didj, 5 d2/dj2."""
+    i, j = coords
+    return {(): 0, (i,): 1, (j,): 2, (i, i): 3, tuple(sorted((i, j))): 4, (j, j): 5}[tuple(alpha)]
 
 
 class _PinnedStage:
@@ -257,6 +288,7 @@ class FusedProblem:
         self.prog_eval = self._upload(tp.prog_eval)
         self.prog_train = self._upload(tp.prog_train)
         self.prog_w = self._upload(tp.prog_w) if tp.wl else None
+        self._setup_fields()
         self._prog_train_ext = None
         self._plan_cache = {}
         self._sizes_cache = {}
@@ -276,6 +308,50 @@ class FusedProblem:
                                       f"(PINNJET_TC=0 runs this problem on the FFMA kernels)")
         if os.environ.get("PINNJET_JIT") == "1":
             self.enable_jit()
+
+    def _setup_fields(self):
+        """Thin-plate-spline groups and field rows of the trace (pde.CustomBoundaryCondition) on the device, as the field
+        kernel's descriptors; the field buffer [n_rows, N] is sized by the batch (``_fields_for``)."""
+        tp = self.tp
+        self.fields, self._field_args = None, None
+        self._retired_fields = []   # smaller field buffers that captured graphs (here or the solvers') may still write
+        if not tp.field_rows:
+            return
+        if len(tp.tps_groups) > PJ_MAX_TPS_GROUPS:
+            raise NotImplementedError(f"{len(tp.tps_groups)} sets of thin-plate-spline centres (the field kernel takes "
+                                      f"{PJ_MAX_TPS_GROUPS})")
+        groups = (PjTpsGroup * len(tp.tps_groups))()
+        keep, local = [], {}
+        for gi, grp in enumerate(tp.tps_groups):
+            maps = [m for m, (g, _) in enumerate(tp.tps_maps) if g == gi]
+            local.update({m: k for k, m in enumerate(maps)})
+            centres = torch.as_tensor(grp["centres"], dtype=self.dtype, device=self.device).contiguous()
+            coefs = torch.as_tensor(np.stack([tp.tps_maps[m][1] for m in maps]), dtype=self.dtype, device=self.device)
+            keep += [centres, coefs]
+            groups[gi] = PjTpsGroup(centres.data_ptr(), coefs.data_ptr(), centres.shape[0], len(maps), grp["coords"][0],
+                                    grp["coords"][1], grp["stiffness"] ** 2)
+        rows = (PjFieldRow * len(tp.field_rows))()
+        for r, (gi, m, alpha) in enumerate(tp.field_rows):
+            rows[r] = PjFieldRow(gi, local[m], field_derivative_code(alpha, tp.tps_groups[gi]["coords"]), 0)
+        self._field_args = (groups, len(tp.tps_groups), rows, len(tp.field_rows), keep)
+
+    def _fields_for(self, ptrs, n):
+        """Field kernel on this call's coordinates; returns the device address of the rows (None without TPS leaves)."""
+        if self._field_args is None:
+            return None
+        groups, n_groups, rows, n_rows, _ = self._field_args
+        if self.fields is None or self.fields.numel() < n_rows * n:
+            # A captured graph -- this problem's or a solver's device loop, replayed after this call -- keeps the address
+            # of the buffer it was captured with, so a buffer is never freed once replaced: growth doubles the size, so
+            # the retired ones together are smaller than the current one.
+            old = 0 if self.fields is None else self.fields.numel()
+            if self.fields is not None:
+                self._retired_fields.append(self.fields)
+            self.fields = torch.empty(max(n_rows * n, 2 * old), dtype=self.dtype, device=self.device)
+        _check(self._fn("pj_tps_fields")(groups, n_groups, rows, n_rows, ptrs, self.tp.n_coords, n, self.fields.data_ptr(),
+                                         self._stream()), "pj_tps_fields")
+        self.kernel_launches += 1
+        return self.fields.data_ptr()
 
     def _fn(self, name):
         """entry point ``name`` of the library, or its float64 twin for a float64 problem"""
@@ -532,7 +608,10 @@ class FusedProblem:
         args = (ctypes.byref(self.spec), self.prog_eval.data_ptr(), self.prog_eval.shape[0], *self._prog_w_args(), ptrs, n,
                 self.pack_buf.data_ptr(), u.data_ptr() if want_u else None, r.data_ptr() if want_residual else None,
                 self.sumsq.data_ptr() if want_sumsq else None, self.workspace.data_ptr(), self.workspace.numel(), self._stream())
-        if self._jit_usable(n):
+        fields = self._fields_for(ptrs, n)
+        if fields is not None:
+            _check(self._fn("pj_forward_fields")(*args[:8], fields, *args[8:]), "pj_forward_fields")
+        elif self._jit_usable(n):
             _check(self.lib.pj_forward_jit(self._jit.function, *args), "pj_forward_jit")
         else:
             _check(self._fn("pj_forward")(*args), "pj_forward")
@@ -579,7 +658,16 @@ class FusedProblem:
             prog = self.enable_function_adjoints()
             prog_len = prog.shape[0]
             rbar = torch.cat([rbar, ubar], dim=0).contiguous()
-        if rbar is None and self._jit_usable(n):   # the problem's own forward kernel (programs compiled in): jit.py
+        fields = self._fields_for(ptrs, n)
+        if fields is not None:
+            _check(self._fn("pj_forward_train_fields")(ctypes.byref(self.spec), prog.data_ptr(), prog_len, *self._prog_w_args(),
+                                                       ptrs, n, self.pack_buf.data_ptr(), fields,
+                                                       (ctypes.c_double if self.f64 else ctypes.c_float)(scale),
+                                                       rbar.data_ptr() if rbar is not None else None,
+                                                       r.data_ptr() if want_residual else None, sumsq_out.data_ptr(),
+                                                       self.workspace.data_ptr(), self.workspace.numel(), self._stream()),
+                   "pj_forward_train_fields")
+        elif rbar is None and self._jit_usable(n):   # the problem's own forward kernel (programs compiled in): jit.py
             _check(self.lib.pj_forward_train_jit(self._jit.function, ctypes.byref(self.spec), prog.data_ptr(), prog_len,
                                                  *self._prog_w_args(), ptrs, n, self.pack_buf.data_ptr(), ctypes.c_float(scale),
                                                  r.data_ptr() if want_residual else None, sumsq_out.data_ptr(),
@@ -624,6 +712,9 @@ class FusedProblem:
                 raise ValueError("the specialised kernel is float32 only (this problem runs in float64)")
             if self._patch_sets:
                 raise ValueError("the program has trainable immediates (Resnet shortcut, equation coefficients)")
+            if self._field_args is not None:
+                raise ValueError("the program reads thin-plate-spline field rows (OP_FIELD), which the specialised kernel "
+                                 "does not compile")
             if any(len(nd.linears) > PJ_MAX_LINEAR for nd in self.tp.nets):
                 raise ValueError(f"a network has more than {PJ_MAX_LINEAR} Linear layers (the tensor-core kernels take at most "
                                  f"{PJ_MAX_LINEAR})")
@@ -762,7 +853,7 @@ class FusedProblem:
         graph, static, stage = st
         self._stage_coords(static, stage, coords)
         graph.replay()
-        self.kernel_launches += 4 if train else 2
+        self.kernel_launches += (4 if train else 2) + (self._field_args is not None)
         return self.sumsq
 
     def train_step_graphed(self, coords, optimizer, n_global=None):
@@ -807,7 +898,7 @@ class FusedProblem:
         self._stage_coords(static, stage, coords)
         graph.replay()
         optimizer._t += 1
-        self.kernel_launches += 5
+        self.kernel_launches += 5 + (self._field_args is not None)
         return self.sumsq
 
     # ---- debugging / tests: raw views of the workspace -----------------------------------------------------------------

@@ -682,7 +682,9 @@ class BaseSolver:
             opt.sync_hyperparameters()
             st.graph.replay()
             opt._t += 1
-            fp.kernel_launches += 6
+            # sampler, K0, K1, K2, K2b, Adam; with thin-plate-spline fields, the field kernel of the step and of every
+            # validation batch
+            fp.kernel_launches += 6 + (getattr(fp, "_field_args", None) is not None) * (1 + self.n_batches["valid"])
             pending += 1
             if callbacks or pending == self.DEVICE_LOOP_CHUNK:     # callbacks read histories / lowest_loss every epoch
                 self._flush_device_loop(st, pending)

@@ -32,6 +32,8 @@ OP_TAN, OP_SINH, OP_COSH, OP_ATAN, OP_ERF = 23, 24, 25, 26, 27
 OP_ST_W = 28   # store a per-point weight of the combined second-order channel
 OP_POW = 29    # slot ** slot: double programs only (an exponent float32 cannot hold, Program.to_f64)
 OP_ST_COT = 30  # add a per-point cotangent dL/d(coefficient k) to the forward kernel's batch sum of coefficient k
+OP_FIELD = 31   # load row `a` of the problem's coordinate-only field table (thin-plate-spline maps) at the point
+MAX_FIELD_ROWS = 64   # field rows per problem (PJ_MAX_FIELD_ROWS of include/pinnjet.h)
 
 _UNARY = {"neg": OP_NEG, "sin": OP_SIN, "cos": OP_COS, "exp": OP_EXP, "log": OP_LOG, "tanh": OP_TANH,
           "sqrt": OP_SQRT, "abs": OP_ABS, "sign": OP_SIGN, "rcp": OP_RCP, "tan": OP_TAN, "sinh": OP_SINH,
@@ -56,6 +58,9 @@ class Graph:
         self.n_sampled = None   # number of sampled coordinates (set by the tracer); constant coordinates follow them
         self.const_coords = []  # values of the constant ("virtual") coordinates n_sampled, n_sampled + 1, ...
         self.coef_tensors = []  # trainable tensors whose elements are coefficients of the trace, in order of first use
+        self.tps_groups = []    # thin-plate-spline centre sets: dict(centres [M, 2] float64, stiffness, coords (i, j))
+        self.tps_maps = []      # (group, coefficients [M + 3] float64) of every distinct TPS map
+        self._tps_keys = {}
 
     def _mk(self, op, args=(), imm=None):
         key = (op, tuple(a.idx for a in args), imm)
@@ -126,6 +131,32 @@ class Graph:
 
     def param(self, k):
         return self._mk("param", (), int(k))
+
+    def tps_group(self, centres, stiffness, coords):
+        """Index of the thin-plate-spline group with these centres [M, 2], stiffness and sampled coordinate indices (i, j),
+        shared by every map over the same centres."""
+        centres = np.ascontiguousarray(centres, dtype=np.float64).reshape(-1, 2)
+        key = ("group", centres.tobytes(), float(stiffness), tuple(int(c) for c in coords))
+        if key not in self._tps_keys:
+            self._tps_keys[key] = len(self.tps_groups)
+            self.tps_groups.append(dict(centres=centres, stiffness=float(stiffness), coords=key[3]))
+        return self._tps_keys[key]
+
+    def tps_map(self, group, coefs):
+        """Index of the TPS map of ``group`` with coefficients [c_1..c_M, c_0, c_x, c_y] (de-duplicated by value)."""
+        coefs = np.ascontiguousarray(coefs, dtype=np.float64).reshape(-1)
+        if coefs.size != self.tps_groups[group]["centres"].shape[0] + 3:
+            raise ValueError("a TPS map needs M + 3 coefficients")
+        key = ("map", int(group), coefs.tobytes())
+        if key not in self._tps_keys:
+            self._tps_keys[key] = len(self.tps_maps)
+            self.tps_maps.append((int(group), coefs))
+        return self._tps_keys[key]
+
+    def tps(self, group, map_idx, alpha=()):
+        """Derivative ``alpha`` (sorted coordinate indices, order <= 2) of TPS map ``map_idx``: a coordinate-only leaf that
+        the kernels read from a field row (OP_FIELD)."""
+        return self._mk("tps", (), (int(group), int(map_idx), tuple(sorted(alpha))))
 
     def register_net(self, module, in_coord):
         key = (id(module), tuple(in_coord))
@@ -794,6 +825,15 @@ def derivative(node, i, memo=None):
             raise ValueError("cannot differentiate a channel-resolved expression")
         elif op == "coord":
             r = g.const(1.0 if n.imm == i else 0.0)
+        elif op == "tps":
+            group, map_idx, alpha = n.imm
+            if i not in g.tps_groups[group]["coords"]:
+                r = g.const(0.0)
+            elif len(alpha) >= 2:
+                raise NotImplementedError("derivative of order 3 of a thin-plate-spline interpolant: the field kernel "
+                                          "evaluates them up to order 2")
+            else:
+                r = g.tps(group, map_idx, alpha + (i,))
         elif op == "net":
             net_idx, o, alpha = n.imm
             r = g.net(net_idx, o, alpha + (i,)) if i in g.nets[net_idx][1] else g.const(0.0)
@@ -892,7 +932,7 @@ def reverse_gradients(roots_and_cotangents, wrt_filter=lambda n: n.op in ("net",
         if wrt_filter(n):
             out[n] = a_bar
             continue
-        if op in ("const", "coord", "rbar", "param", "theta", "net", "ych", "sign"):
+        if op in ("const", "coord", "rbar", "param", "theta", "net", "ych", "sign", "tps"):
             continue
         if op == "add":
             acc(n.args[0], a_bar)
@@ -1149,8 +1189,9 @@ def _f64_of_words(lo, hi):
     return float(np.array([lo, hi], dtype=np.int32).view(np.float64)[0])
 
 
-def lower(outputs, yrow_of):
-    """``outputs``: list of (store_op, index, Sym).  ``yrow_of(net, out, channel_alpha) -> row`` in the y table.
+def lower(outputs, yrow_of, field_row_of=None):
+    """``outputs``: list of (store_op, index, Sym).  ``yrow_of(net, out, channel_alpha) -> row`` in the y table,
+    ``field_row_of(tps leaf imm) -> row`` in the field table.
 
     Emits instructions in topological order with liveness-based slot reuse (so that the interpreter's per-thread
     value file is small enough for shared memory)."""
@@ -1187,6 +1228,8 @@ def lower(outputs, yrow_of):
             code.append((OP_CONST, dst, 0, 0))
         elif op == "coord":
             code.append((OP_COORD, dst, n.imm, 0))
+        elif op == "tps":
+            code.append((OP_FIELD, dst, field_row_of(n.imm), 0))
         elif op == "ych":
             code.append((OP_NET, dst, yrow_of(*n.imm), 0))
         elif op == "net":
@@ -1214,11 +1257,13 @@ def depends_on_jets(expr):
     return any(n.op in ("net", "ych") for n in topo_order([expr]))
 
 
-def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n_seed=0, n_w=0, theta=None, n_cot=0):
+def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n_seed=0, n_w=0, theta=None, n_cot=0,
+                     fields=None):
     """Pure-numpy interpreter of the bytecode (host-side check of the lowering; float64).  ``theta``: values of the
     trainable scalars the program's patched constants stand for (``Program.patch`` keys -> float).  Float programs take
     their immediates from ``exact_imm``; double programs (``Program.to_f64``) are decoded from the code alone.
-    ``n_cot > 0``: also return the per-point coefficient cotangents [n_cot, N] (OP_ST_COT) as a fourth result."""
+    ``n_cot > 0``: also return the per-point coefficient cotangents [n_cot, N] (OP_ST_COT) as a fourth result.
+    ``fields``: the field rows [n_rows, N] that OP_FIELD reads."""
     n = coords.shape[1]
     val = np.zeros((program.n_slots, n))
     u, r, seed = np.zeros((n_u, n)), np.zeros((n_r, n)), np.zeros((n_seed, n))
@@ -1238,6 +1283,8 @@ def evaluate_program(program, coords, y, rbar=None, params=None, n_u=0, n_r=0, n
             val[dst] = coords[a]
         elif op == OP_NET:
             val[dst] = y[a]
+        elif op == OP_FIELD:
+            val[dst] = fields[a]
         elif op == OP_RBAR:
             val[dst] = rbar[a]
         elif op == OP_PARAM:

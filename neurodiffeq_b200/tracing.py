@@ -214,12 +214,31 @@ class TracedProblem:
                 self.coef_index[("coef", id(t), i)] = off + i
             off += t.numel()
         self.n_coef = off
-        self.prog_w = S.lower([(S.OP_ST_W, row, e) for row, e in self.weight_exprs], yrow) if self.wl else None
+        self._build_field_table()
+        self.prog_w = (S.lower([(S.OP_ST_W, row, e) for row, e in self.weight_exprs], yrow, self._field_row)
+                       if self.wl else None)
         # --- programs ---------------------------------------------------------------------------------------------------
         self.prog_eval = S.lower([(S.OP_ST_U, k, f) for k, f in enumerate(self.funcs)]
-                                 + [(S.OP_ST_R, e, r) for e, r in enumerate(self.residuals)], yrow)
+                                 + [(S.OP_ST_R, e, r) for e, r in enumerate(self.residuals)], yrow, self._field_row)
         self.prog_train = self._train_program(external_rbar=False)
         self._prog_train_ext = None
+
+    def _build_field_table(self):
+        """Thin-plate-spline leaves (pde.CustomBoundaryCondition) -> the field table the field kernel fills before the
+        forward kernel runs: ``tps_groups`` (centres, stiffness, coordinate indices), ``tps_maps`` (group, coefficients)
+        and ``field_rows``, one (group, map, alpha) per distinct leaf, which OP_FIELD reads by index."""
+        g = self.graph
+        exprs = self.funcs + self.residuals + [e for _, e in self.weight_exprs]
+        leaves = sorted({n.imm for n in S.topo_order(exprs) if n.op == "tps"})
+        if len(leaves) > S.MAX_FIELD_ROWS:
+            raise NotImplementedError(f"{len(leaves)} thin-plate-spline field rows (the field kernel and the engine take "
+                                      f"at most {S.MAX_FIELD_ROWS})")
+        self.tps_groups, self.tps_maps = list(g.tps_groups), list(g.tps_maps)
+        self.field_rows = leaves
+        self._field_index = {imm: k for k, imm in enumerate(leaves)}
+
+    def _field_row(self, imm):
+        return self._field_index[imm]
 
     def _mergeable_constant_coords(self):
         """Constant coordinates (boundary abscissae) that never feed the same network instance can share one jet
@@ -294,7 +313,7 @@ class TracedProblem:
         # per-point cotangents of the coefficients; the forward kernel sums them over the batch
         outs += sorted(((S.OP_ST_COT, self.coef_index[leaf.imm], expr) for leaf, expr in adj.items() if is_coef(leaf)),
                        key=lambda o: o[1])
-        return S.lower(outs, self._yrow)
+        return S.lower(outs, self._yrow, self._field_row)
 
     @property
     def prog_train_ext(self):

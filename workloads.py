@@ -684,6 +684,95 @@ def _i4(nd):
                     make_nets, make_conditions, diff_eqs, 1, 1024, _fcnn_flops(shape, 3), None, make_coefficients)
 
 
+# ----------------------------------------------------------------------------------------------------------------------
+# G1, G2  irregular 2-D domains: CustomBoundaryCondition (Dirichlet control points, thin-plate-spline fields).  Their
+# points come from sample_in_domain, not from the whole box.
+# ----------------------------------------------------------------------------------------------------------------------
+def star_control_points(nd, value):
+    """The hexagram of the reference's getting-started notebook: 12 edges of 10 steps from (0, -1), turning left and right
+    in turn, so 120 control points with the boundary values value(x, y)."""
+    edge_length = 2.0 / np.sin(np.pi / 3) / 4
+    step = edge_length / 10
+    direction, x, y, points = np.pi * 2 / 3, 0.0, -1.0, []
+    for edge in range(12):
+        for _ in range(10):
+            points.append(nd.DirichletControlPoint(loc=(x, y), val=value(x, y)))
+            x += step * np.cos(direction)
+            y += step * np.sin(direction)
+        direction += np.pi / 3 if edge % 2 == 0 else -np.pi * 2 / 3
+    return points
+
+
+def l_shape_control_points(nd, value, per_unit=8):
+    """The L-shape [-1, 1] x [-1, 0] u [-1, 0] x [0, 1] (non-convex, star-shaped about (-0.5, -0.5)): per_unit points per
+    unit of edge length, walked from (-1, -1) counter-clockwise."""
+    corners = [(-1.0, -1.0), (1.0, -1.0), (1.0, 0.0), (0.0, 0.0), (0.0, 1.0), (-1.0, 1.0), (-1.0, -1.0)]
+    points = []
+    for (x0, y0), (x1, y1) in zip(corners[:-1], corners[1:]):
+        steps = int(round(per_unit * (abs(x1 - x0) + abs(y1 - y0))))
+        for k in range(steps):
+            x, y = x0 + (x1 - x0) * k / steps, y0 + (y1 - y0) * k / steps
+            points.append(nd.DirichletControlPoint(loc=(x, y), val=value(x, y)))
+    return points
+
+
+def _g1(nd):
+    """The getting-started notebook's "Irregular Domain" example as written: `de_star`, u_xx + u_yy + exp(u) = 1 + x^2 + y^2
+    + 4 / (1 + x^2 + y^2)^2 on the hexagram, u = log(1 + x^2 + y^2) at its 120 control points, FCNN(2, 1, (40, 40), ELU)."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(40, 40), actv=torch.nn.ELU)]
+
+    def make_conditions():
+        return [nd.CustomBoundaryCondition(center_point=nd.Point((0.0, 0.0)), dirichlet_control_points=star_control_points(
+            nd, lambda x, y: np.log(1 + x ** 2 + y ** 2)))]
+
+    def diff_eqs(u, x, y):
+        return [nd.diff(u, x, order=2) + nd.diff(u, y, order=2) + torch.exp(u) - 1.0 - x ** 2 - y ** 2
+                - 4.0 / (1.0 + x ** 2 + y ** 2) ** 2]
+
+    return Workload("g1_star_de_star", "Solver2D", ("x", "y"), ((-1.0, 1.0), (-1.0, 1.0)), [((2, 40, 40, 1), "elu")],
+                    make_nets, make_conditions, diff_eqs, 1, 16384, _fcnn_flops((2, 40, 40, 1), 4), None)
+
+
+def _g2(nd):
+    """Two functions on the L-shape, each with its own CustomBoundaryCondition on the same control-point locations
+    (u = x y, v = cos(x + y) there): the length-factor maps are shared, the A_D maps are not.  The coupled residuals have a
+    mixed partial u_xy and a second derivative with a jet-dependent coefficient, u v_xx, so the problem keeps separate
+    second-order channels and needs the mixed second derivatives of the fields."""
+    def make_nets():
+        return [nd.FCNN(n_input_units=2, n_output_units=1, hidden_units=(32, 32)) for _ in range(2)]
+
+    def make_conditions():
+        center = nd.Point((-0.5, -0.5))
+        return [nd.CustomBoundaryCondition(center, l_shape_control_points(nd, lambda x, y: x * y)),
+                nd.CustomBoundaryCondition(center, l_shape_control_points(nd, lambda x, y: np.cos(x + y)))]
+
+    def diff_eqs(u, v, x, y):
+        u_x = nd.diff(u, x)
+        return [nd.diff(u, x, order=2) + nd.diff(u, y, order=2) + 0.5 * nd.diff(u_x, y) - v - x * y,
+                u * nd.diff(v, x, order=2) + nd.diff(v, y, order=2) + torch.sin(u) - 1.0]
+
+    shape = (2, 32, 32, 1)
+    return Workload("g2_l_shape_coupled", "Solver2D", ("x", "y"), ((-1.0, 1.0), (-1.0, 1.0)), [(shape, "tanh")] * 2,
+                    make_nets, make_conditions, diff_eqs, 2, 16384, 2 * _fcnn_flops(shape, 7), None)
+
+
+def sample_in_domain(workload, n, seed=0):
+    """Like sample_coords, for the irregular workloads: float32 points [2, n] drawn uniformly in the box and kept where the
+    first condition's eager ``in_domain`` (float64) says they are inside, in draw order; deterministic per seed."""
+    cond = workload.make_conditions()[0]
+    rs = np.random.RandomState(seed)
+    (x0, x1), (y0, y1) = workload.coord_ranges
+    kept = []
+    while sum(k.shape[1] for k in kept) < n:
+        cand = np.stack([(x0 + (x1 - x0) * rs.rand(4 * n + 64)).astype(np.float32),
+                         (y0 + (y1 - y0) * rs.rand(4 * n + 64)).astype(np.float32)])
+        t = torch.from_numpy(cand.astype(np.float64))
+        inside = np.asarray(cond.in_domain(t[0].reshape(-1, 1), t[1].reshape(-1, 1))).reshape(-1)
+        kept.append(cand[:, inside])
+    return np.concatenate(kept, axis=1)[:, :n]
+
+
 _EXTRA = {
     "x1": lambda nd: _heat(nd, "x1_heat_dirichlet_neumann", "right"),
     "x2": lambda nd: _heat(nd, "x2_heat_neumann_dirichlet", "left"),
@@ -732,6 +821,10 @@ _BUILDERS.update(_DEEP)
 _INVERSE = {"i1": _i1, "i2": _i2, "i3": _i3, "i4": _i4}
 INVERSE_NAMES = tuple(_INVERSE)
 _BUILDERS.update(_INVERSE)
+# irregular domains (pde.CustomBoundaryCondition, points from sample_in_domain); kept out of the tuples above as well
+_IRREGULAR = {"g1": _g1, "g2": _g2}
+IRREGULAR_NAMES = tuple(_IRREGULAR)
+_BUILDERS.update(_IRREGULAR)
 # workloads whose conditions see only the first coordinate (a network of r alone, as SolverSpherical passes it)
 _RADIAL = ("s1", "s2")
 
@@ -799,6 +892,7 @@ def product_namespace():
     from neurodiffeq_b200.networks import FCNN, SinActv, Resnet
     from neurodiffeq_b200 import conditions as c
     from neurodiffeq_b200 import function_basis as fb
+    from neurodiffeq_b200 import pde
     return types.SimpleNamespace(
         diff=diff, FCNN=FCNN, Resnet=Resnet, SinActv=SinActv, IVP=c.IVP, BundleIVP=c.BundleIVP, DirichletBVP2D=c.DirichletBVP2D,
         IBVP1D=c.IBVP1D, DirichletBVPSpherical=c.DirichletBVPSpherical, NoCondition=c.NoCondition,
@@ -806,7 +900,8 @@ def product_namespace():
         spherical_laplacian=ops.spherical_laplacian, laplacian=ops.laplacian, grad=ops.grad, div=ops.div,
         curl=ops.curl, DirichletBVPSphericalBasis=c.DirichletBVPSphericalBasis,
         InfDirichletBVPSphericalBasis=c.InfDirichletBVPSphericalBasis, HarmonicsLaplacian=fb.HarmonicsLaplacian,
-        RealSphericalHarmonics=fb.RealSphericalHarmonics)
+        RealSphericalHarmonics=fb.RealSphericalHarmonics, CustomBoundaryCondition=pde.CustomBoundaryCondition,
+        Point=pde.Point, DirichletControlPoint=pde.DirichletControlPoint)
 
 
 def distinct(nets):
