@@ -325,6 +325,58 @@ int pj_adam_step(float* theta, const float* grad, float* exp_avg, float* exp_avg
                  float beta1, float beta2, float eps, const float* loss /*device or NULL*/, float* best_loss, float* best_theta,
                  void* stream);
 
+/* ---- L-BFGS on the flat parameter buffer, one launch per function evaluation (optim.FlatLBFGS) ----------------------
+ * torch.optim.LBFGS (reference solvers.py:22-32, 369-400) with its order of operations, run on one thread-block cluster
+ * (pj_lbfgs_shape: 1..16 CTAs from n_theta).  Call it after every closure evaluation with grad = dL/dtheta there (or the
+ * gradient the line search returns) and *loss = its loss (a device scalar, or NULL and loss_host).  One launch:
+ *   1. PJ_LBFGS_LINE_SEARCH without PJ_LBFGS_ENTRY (the call after a line search): theta += t_ls * dir, the step the
+ *      search chose, and t = t_ls;
+ *   2. max|g|, |g|_1, max|t dir|, and the tests that end torch's iteration loop (PJ_LBFGS_ENTRY: the first evaluation of a
+ *      step, where only max|g| <= tolerance_grad is tested); PJ_LBFGS_MAY_CONTINUE clear means the iteration or
+ *      evaluation budget is spent.  On a stop the launch ends here with status[PJ_LBFGS_STOP] = the reason;
+ *   3. the next iteration: y = g - grad_prev, s = t dir; if y.s > 1e-10 the pair enters the ring of history_size slots
+ *      (old_dirs = y, old_stps = s, rho = 1/y.s, overwriting the oldest) and H_diag = y.s / y.y; grad_prev = g; the
+ *      two-loop recursion dir = -H g; t = lr (first iteration: min(1, 1/|g|_1) lr); gtd = g.dir; if gtd > -tolerance_change
+ *      status[PJ_LBFGS_STOP] = PJ_LBFGS_STOP_DESCENT, else without PJ_LBFGS_LINE_SEARCH theta += t dir (with it, the
+ *      caller searches along dir from status[PJ_LBFGS_T]).
+ * The state between calls is the caller's buffers: dir, grad_prev [n]; old_dirs, old_stps [history_size][n]; rho
+ * [history_size]; status = PJ_LBFGS_STATUS device doubles, zero before the first call (n_iter 0 = no iteration yet).
+ * Float or double (_f64) throughout; no allocation, no host synchronisation; the result is run-to-run identical. */
+#define PJ_LBFGS_MAX_HISTORY 2048
+#define PJ_LBFGS_ENTRY 1
+#define PJ_LBFGS_LINE_SEARCH 2
+#define PJ_LBFGS_MAY_CONTINUE 4
+#define PJ_LBFGS_STATUS 16
+#define PJ_LBFGS_N_ITER 0       /* iterations so far (torch: state["n_iter"])                                           */
+#define PJ_LBFGS_FUNC_EVALS 1   /* sum of n_evals (torch: state["func_evals"])                                          */
+#define PJ_LBFGS_NUM_OLD 2      /* pairs in the ring                                                                    */
+#define PJ_LBFGS_HEAD 3         /* slot of the oldest pair                                                              */
+#define PJ_LBFGS_H_DIAG 4
+#define PJ_LBFGS_T 5            /* step length of dir (the next iteration's s = t dir)                                  */
+#define PJ_LBFGS_GTD 6
+#define PJ_LBFGS_LOSS 7         /* loss of the last call                                                                */
+#define PJ_LBFGS_PREV_LOSS 8    /* loss at the start of the last iteration                                              */
+#define PJ_LBFGS_STOP 9         /* PJ_LBFGS_RUNNING or why the loop ends                                                */
+#define PJ_LBFGS_GMAX 10        /* max|g|                                                                               */
+#define PJ_LBFGS_G1 11          /* |g|_1                                                                                */
+#define PJ_LBFGS_TDMAX 12       /* max|t dir| of the step just taken                                                    */
+#define PJ_LBFGS_YS 13          /* y.s of the last history update                                                       */
+#define PJ_LBFGS_RUNNING 0
+#define PJ_LBFGS_STOP_GRAD 1    /* max|g| <= tolerance_grad                                                             */
+#define PJ_LBFGS_STOP_LIMIT 2   /* PJ_LBFGS_MAY_CONTINUE clear                                                          */
+#define PJ_LBFGS_STOP_STEP 3    /* max|t dir| <= tolerance_change                                                       */
+#define PJ_LBFGS_STOP_LOSS 4    /* |loss - prev_loss| < tolerance_change                                                */
+#define PJ_LBFGS_STOP_DESCENT 5 /* gtd > -tolerance_change: the iteration started but takes no step                     */
+int pj_lbfgs_shape(int64_t n_theta, int32_t* cluster, int32_t* threads);
+int pj_lbfgs_step(float* theta, const float* grad, float* dir, float* grad_prev, float* old_dirs, float* old_stps, float* rho,
+                  int64_t n, int32_t history_size, double* status /*device*/, const float* loss /*device or NULL*/,
+                  double loss_host, double lr, double tolerance_grad, double tolerance_change, double t_ls, int32_t flags,
+                  int32_t n_evals, void* stream);
+int pj_lbfgs_step_f64(double* theta, const double* grad, double* dir, double* grad_prev, double* old_dirs, double* old_stps,
+                      double* rho, int64_t n, int32_t history_size, double* status, const double* loss, double loss_host,
+                      double lr, double tolerance_grad, double tolerance_change, double t_ls, int32_t flags, int32_t n_evals,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

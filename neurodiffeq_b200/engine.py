@@ -130,8 +130,14 @@ def load_library():
     lib.pj_forward_fields_f64.argtypes = lib.pj_forward_fields.argtypes
     lib.pj_forward_train_fields.argtypes = lib.pj_forward_train.argtypes[:8] + [vp] + lib.pj_forward_train.argtypes[8:]
     lib.pj_forward_train_fields_f64.argtypes = [ctypes.c_double if t is f32 else t for t in lib.pj_forward_train_fields.argtypes]
+    # L-BFGS on the flat parameter buffer (optim.FlatLBFGS)
+    f64 = ctypes.c_double
+    lib.pj_lbfgs_shape.argtypes = [i64, ctypes.POINTER(i32), ctypes.POINTER(i32)]
+    lib.pj_lbfgs_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, i32, vp, vp, f64, f64, f64, f64, f64, i32, i32, vp]
+    lib.pj_lbfgs_step_f64.argtypes = lib.pj_lbfgs_step.argtypes
     for fn in (lib.pj_tps_fields, lib.pj_tps_fields_f64, lib.pj_forward_fields, lib.pj_forward_fields_f64,
-               lib.pj_forward_train_fields, lib.pj_forward_train_fields_f64):
+               lib.pj_forward_train_fields, lib.pj_forward_train_fields_f64, lib.pj_lbfgs_shape, lib.pj_lbfgs_step,
+               lib.pj_lbfgs_step_f64):
         fn.restype = ctypes.c_int
     for fn in (lib.pj_sizes, lib.pj_pack, lib.pj_forward, lib.pj_forward_train, lib.pj_backward, lib.pj_forward_jit,
                lib.pj_forward_train_jit, lib.pj_backward_allreduce, lib.pj_sizes_f64, lib.pj_plan_info_f64, lib.pj_pack_f64,
@@ -146,7 +152,7 @@ def load_library():
 EXPORTED_SYMBOLS = ("pj_abi_version", "pj_last_error", "pj_sizes", "pj_plan_info", "pj_pack", "pj_forward", "pj_forward_train",
                     "pj_backward", "pj_allreduce_bytes", "pj_allreduce_oneshot", "pj_sample", "pj_adam_step", "pj_forward_jit",
                     "pj_forward_train_jit", "pj_backward_allreduce_bytes", "pj_backward_allreduce", "pj_pack_zero",
-                    "pj_tps_fields", "pj_forward_fields", "pj_forward_train_fields")
+                    "pj_tps_fields", "pj_forward_fields", "pj_forward_train_fields", "pj_lbfgs_shape", "pj_lbfgs_step")
 F64_SYMBOLS = ("pj_sizes_f64", "pj_plan_info_f64", "pj_pack_f64", "pj_pack_zero_f64", "pj_forward_f64", "pj_forward_train_f64",
                "pj_backward_f64")
 
